@@ -127,11 +127,19 @@ SIGNATURES = {
     "mb200_peer_put_all": ("i", "pqpqip"),
     "mb200_peer_reduce_put_i64": ("i", "pqqqiiip"),
 }
+# The calibration-error entry points (K14) are declared in the companion header include/metrics_b200_calibration.h and
+# exported from the same library; tests/test_calibration_abi.py holds this table to that header.
+CALIBRATION_SIGNATURES = {
+    "mb200_calibration_scratch_bytes": ("q", "q"),
+    "mb200_calibration_top_label": ("i", "pipiqqiqpppqpp"),
+    "mb200_calibration_bin_scratch_bytes": ("q", "qq"),
+    "mb200_calibration_bin_sums": ("i", "pipiqpqppppqp"),
+}
 
 
 def declare_signatures(handle) -> None:
     """Set ``restype`` / ``argtypes`` of every exported function on a loaded library handle."""
-    for name, (ret, args) in SIGNATURES.items():
+    for name, (ret, args) in (*SIGNATURES.items(), *CALIBRATION_SIGNATURES.items()):
         fn = getattr(handle, name)
         fn.restype = _C_TYPES[ret]
         fn.argtypes = [_C_TYPES[a] for a in args]
@@ -881,3 +889,61 @@ def curve_evaluate_multilabel(preds: Tensor, target: Tensor, num_labels: int, ig
         )
     check(rc, "curve_evaluate_multilabel")
     return auroc, ap, counts, curve
+
+
+# ----------------------------------------------------------------------------------------------------------
+# K14 wrappers (calibration error, include/metrics_b200_calibration.h)
+# ----------------------------------------------------------------------------------------------------------
+def calibration_top_label(preds: Tensor, target: Tensor, ignore_index: Optional[int] = None,
+                          err_flag: Optional[Tensor] = None) -> tuple[Tensor, Tensor]:
+    """K14a (``mb200_calibration_top_label``): ``normalize_logits_if_needed(preds, "softmax").max(dim=1)`` and the
+    ``argmax == target`` hit of every row of ``preds [N, C]`` / ``target [N]``, from one read of ``preds``.  Returns float32
+    ``(confidence [N], accuracy [N])``; rows whose target is ``ignore_index`` take no part in the logits vote and hold
+    zeros.  No host synchronisation."""
+    dev = require_cuda(preds, target)
+    preds = preds.contiguous()
+    target = target.contiguous()
+    n, c = preds.shape
+    conf = torch.empty(n, dtype=torch.float32, device=dev)
+    acc = torch.empty(n, dtype=torch.float32, device=dev)
+    if n == 0:
+        return conf, acc
+    lib_ = lib()
+    nbytes = int(lib_.mb200_calibration_scratch_bytes(n))
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    with on_device(dev):
+        rc = lib_.mb200_calibration_top_label(
+            preds.data_ptr(), tag(preds), target.data_ptr(), tag(target), n, c, int(ignore_index is not None),
+            int(ignore_index or 0), conf.data_ptr(), acc.data_ptr(), scratch.data_ptr(), nbytes, ptr(err_flag),
+            stream_handle(dev),
+        )
+    if rc:
+        check(rc, "calibration_top_label")
+    return conf, acc
+
+
+def calibration_bin_sums(confidences: Tensor, accuracies: Tensor, boundaries: Tensor) -> tuple[Tensor, Tensor, Tensor]:
+    """K14b (``mb200_calibration_bin_sums``): per slot of ``torch.bucketize(confidences, boundaries, right=True) - 1`` the
+    exact count (int64) and the float64 sums of the confidences and of the accuracies (rounded to the confidence dtype
+    first).  ``boundaries`` holds ``n_bins + 1`` values in the confidence dtype; all three outputs have ``n_bins + 1`` slots.
+    Deterministic: same inputs, same bits."""
+    dev = require_cuda(confidences, accuracies, boundaries)
+    confidences = confidences.contiguous()
+    accuracies = accuracies.contiguous()
+    boundaries = boundaries.contiguous()
+    n, slots = confidences.numel(), boundaries.numel()
+    count = torch.empty(slots, dtype=torch.int64, device=dev)
+    sum_conf = torch.empty(slots, dtype=torch.float64, device=dev)
+    sum_acc = torch.empty(slots, dtype=torch.float64, device=dev)
+    lib_ = lib()
+    nbytes = int(lib_.mb200_calibration_bin_scratch_bytes(n, slots - 1))
+    scratch = torch.empty(max(nbytes, 0), dtype=torch.uint8, device=dev)
+    with on_device(dev):
+        rc = lib_.mb200_calibration_bin_sums(
+            confidences.data_ptr(), tag(confidences), accuracies.data_ptr(), tag(accuracies), n, boundaries.data_ptr(),
+            slots - 1, count.data_ptr(), sum_conf.data_ptr(), sum_acc.data_ptr(), scratch.data_ptr(), nbytes,
+            stream_handle(dev),
+        )
+    if rc:
+        check(rc, "calibration_bin_sums")
+    return count, sum_conf, sum_acc

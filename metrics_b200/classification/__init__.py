@@ -89,3 +89,8 @@ from metrics_b200.classification.at_fixed import (  # noqa: F401,E402
 from metrics_b200.classification.exact_match import ExactMatch, MulticlassExactMatch, MultilabelExactMatch  # noqa: F401,E402
 from metrics_b200.classification.logauc import BinaryLogAUC, LogAUC, MulticlassLogAUC, MultilabelLogAUC  # noqa: F401,E402
 from metrics_b200.classification.group_fairness import BinaryFairness, BinaryGroupStatRates  # noqa: F401,E402
+from metrics_b200.classification.calibration_error import (  # noqa: F401,E402
+    BinaryCalibrationError,
+    CalibrationError,
+    MulticlassCalibrationError,
+)

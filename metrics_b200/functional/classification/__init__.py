@@ -101,6 +101,11 @@ from metrics_b200.functional.classification.at_fixed import (  # noqa: F401,E402
     sensitivity_at_specificity,
     specificity_at_sensitivity,
 )
+from metrics_b200.functional.classification.calibration_error import (  # noqa: F401,E402
+    binary_calibration_error,
+    calibration_error,
+    multiclass_calibration_error,
+)
 
 # The reference's import paths `<package>.{cohen_kappa, matthews_corrcoef, negative_predictive_value, specificity}` are alias submodules that share a name with a function exported
 # above.  Loading a submodule binds it as a package attribute, so load them now and re-bind the functions afterwards: a
