@@ -684,19 +684,31 @@ REG_MSE, REG_MAE, REG_MAPE, REG_SMAPE, REG_WMAPE, REG_MSLE, REG_LOGCOSH, REG_MIN
 _REG_NUM_SUMS = {REG_WMAPE: 2, REG_R2: 3, REG_EXPVAR: 4, REG_TWEEDIE: 4}
 
 
+def regression_compute_dtype(preds: Tensor, target: Tensor) -> torch.dtype:
+    """The dtype the regression terms are computed in: the promoted dtype of the two inputs, as in the reference's
+    ``preds - target``; float32 when neither input is floating point."""
+    dtype = torch.promote_types(preds.dtype, target.dtype)
+    return dtype if dtype.is_floating_point else torch.float32
+
+
 def regression_sums(preds: Tensor, target: Tensor, op: int, num_outputs: int = 1, param: float = 0.0, eps: float = 0.0) -> Tensor:
-    """``float64 [num_sums, num_outputs]`` sums of the per-element terms of regression op ``op`` (``mb200_regression_sums``)."""
+    """``float64 [num_sums, num_outputs]`` sums of the per-element terms of regression op ``op`` (``mb200_regression_sums``)
+    over the ``[numel / num_outputs, num_outputs]`` row-major view of the inputs.  The terms are computed in
+    `regression_compute_dtype`; only an input of another dtype is cast."""
     dev = require_cuda(preds, target)
-    if not preds.is_floating_point():
-        preds = preds.float()
-    if target.dtype != preds.dtype:
-        target = target.to(preds.dtype)
+    d = int(num_outputs)
+    if d < 1 or preds.numel() % d:
+        raise ValueError(f"regression_sums: {preds.numel()} elements do not split into rows of num_outputs={d}")
+    dtype = regression_compute_dtype(preds, target)
+    if preds.dtype != dtype:
+        preds = preds.to(dtype)
+    if target.dtype != dtype:
+        target = target.to(dtype)
     if _TORCH_BINDING:
-        return _ops().regression_sums(preds, target, int(op), int(num_outputs), float(param), float(eps))
+        return _ops().regression_sums(preds, target, int(op), d, float(param), float(eps))
     preds = preds.contiguous()
     target = target.contiguous()
-    d = int(num_outputs)
-    n = preds.numel() // d if d else 0
+    n = preds.numel() // d
     k = _REG_NUM_SUMS.get(op, 1)
     out = torch.empty((k, d), dtype=torch.float64, device=dev)
     lib_ = lib()

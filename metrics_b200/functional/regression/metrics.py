@@ -5,6 +5,7 @@ by ONE kernel pass instead of 2-5 elementwise/reduction launches; the `_x_comput
 """
 from __future__ import annotations
 
+import math
 from typing import Optional, Union
 
 import torch
@@ -18,25 +19,24 @@ from metrics_b200.utilities.exceptions import TorchMetricsUserError
 _EPS = 1.17e-06
 
 
-def _out_dtype(preds: Tensor) -> torch.dtype:
-    return preds.dtype if preds.is_floating_point() else torch.float32
-
-
 def _sums(preds: Tensor, target: Tensor, op: int, num_outputs: int = 1, param: float = 0.0, eps: float = 0.0) -> Tensor:
-    return _native.regression_sums(preds, target, op, num_outputs, param, eps).to(_out_dtype(preds))
+    """The op's sums in the dtype the reference's ``preds - target`` has (the promoted dtype of the inputs)."""
+    return _native.regression_sums(preds, target, op, num_outputs, param, eps).to(_native.regression_compute_dtype(preds, target))
 
 
-def _flat_or_cols(preds: Tensor, num_outputs: int) -> int:
-    return 1 if num_outputs == 1 else num_outputs
+def _dim0_sums(preds: Tensor, target: Tensor, op: int) -> list[Tensor]:
+    """Each of the op's sums over dim 0 only, shaped ``preds.shape[1:]`` (the reference's ``torch.sum(..., dim=0)``): the
+    kernel sees the inputs as ``[shape[0], prod(shape[1:])]``."""
+    s = _sums(preds, target, op, math.prod(preds.shape[1:]))
+    return [row.reshape(preds.shape[1:]) for row in s]
 
 
 # ---- MSE (mse.py:22-58) ----------------------------------------------------------------------------------------------
 def _mean_squared_error_update(preds: Tensor, target: Tensor, num_outputs: int) -> tuple[Tensor, int]:
     _check_same_shape(preds, target)
-    s = _sums(preds, target, _native.REG_MSE, _flat_or_cols(preds, num_outputs))[0]
     if num_outputs == 1:
-        return s.reshape(()), target.numel()
-    return s, target.shape[0]
+        return _sums(preds, target, _native.REG_MSE)[0].reshape(()), target.numel()
+    return _dim0_sums(preds, target, _native.REG_MSE)[0], target.shape[0]
 
 
 def _mean_squared_error_compute(sum_squared_error: Tensor, num_obs: Union[int, Tensor], squared: bool = True) -> Tensor:
@@ -51,10 +51,9 @@ def mean_squared_error(preds: Tensor, target: Tensor, squared: bool = True, num_
 # ---- MAE (mae.py:22-60) ----------------------------------------------------------------------------------------------
 def _mean_absolute_error_update(preds: Tensor, target: Tensor, num_outputs: int = 1) -> tuple[Tensor, int]:
     _check_same_shape(preds, target)
-    s = _sums(preds, target, _native.REG_MAE, _flat_or_cols(preds, num_outputs))[0]
     if num_outputs == 1:
-        return s.reshape(()), target.numel()
-    return s, target.shape[0]
+        return _sums(preds, target, _native.REG_MAE)[0].reshape(()), target.numel()
+    return _dim0_sums(preds, target, _native.REG_MAE)[0], target.shape[0]
 
 
 def _mean_absolute_error_compute(sum_abs_error: Tensor, num_obs: Union[int, Tensor]) -> Tensor:
@@ -170,11 +169,8 @@ def _r2_score_update(preds: Tensor, target: Tensor) -> tuple[Tensor, Tensor, Ten
             "Expected both prediction and target to be 1D or 2D tensors,"
             f" but received tensors with dimension {preds.shape}"
         )
-    d = 1 if preds.ndim == 1 else preds.shape[1]
-    s = _sums(preds, target, _native.REG_R2, d)
-    if preds.ndim == 1:
-        return s[0, 0], s[1, 0], s[2, 0], target.size(0)
-    return s[0], s[1], s[2], target.size(0)
+    sum_squared_obs, sum_obs, rss = _dim0_sums(preds, target, _native.REG_R2)
+    return sum_squared_obs, sum_obs, rss, target.size(0)
 
 
 def _r2_score_compute(
@@ -240,11 +236,8 @@ def relative_squared_error(preds: Tensor, target: Tensor, squared: bool = True) 
 # ---- Explained variance (explained_variance.py:25-110) ----------------------------------------------------------------
 def _explained_variance_update(preds: Tensor, target: Tensor) -> tuple[int, Tensor, Tensor, Tensor, Tensor]:
     _check_same_shape(preds, target)
-    d = 1 if preds.ndim == 1 else preds.shape[1]
-    s = _sums(preds.reshape(preds.shape[0], -1), target.reshape(target.shape[0], -1), _native.REG_EXPVAR, d)
-    if preds.ndim == 1:
-        return preds.size(0), s[0, 0], s[1, 0], s[2, 0], s[3, 0]
-    return preds.size(0), s[0], s[1], s[2], s[3]
+    sum_error, sum_squared_error, sum_target, sum_squared_target = _dim0_sums(preds, target, _native.REG_EXPVAR)
+    return preds.size(0), sum_error, sum_squared_error, sum_target, sum_squared_target
 
 
 def _explained_variance_compute(
@@ -305,7 +298,7 @@ def _tweedie_deviance_score_update(preds: Tensor, targets: Tensor, power: float 
             raise ValueError(f"For power={power}, 'targets' has to be strictly positive and 'preds' cannot be negative.")
     elif bad_preds or neg_targets or zero_targets:
         raise ValueError(f"For power={power}, both 'preds' and 'targets' have to be strictly positive.")
-    return sums[0].to(_out_dtype(preds)), num_observations
+    return sums[0].to(_native.regression_compute_dtype(preds, targets)), num_observations
 
 
 def _tweedie_deviance_score_compute(sum_deviance_score: Tensor, num_observations: Tensor) -> Tensor:

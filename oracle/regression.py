@@ -101,6 +101,68 @@ def tweedie_deviance_score(p, t, power=0.0):  # tweedie_deviance.py:22-143 (doma
     return dev.sum() / dev.size
 
 
+# ---- the kernel's per-element terms (K9, csrc/regression_terms.cuh) ---------------------------------------------------
+# `terms32` restates `reg_terms` operation for operation in the kernel's term precision: float32 for float32 / float16 /
+# bfloat16 inputs (upcast exactly), float64 for float64 inputs.  For ops 0-4, 8 and 9 (MSE, MAE, MAPE, SMAPE, WMAPE, R2,
+# EV) every operation is an IEEE-exact one (-, *, /, fabs, fmax), so these terms are bit-identical to the kernel's; the
+# transcendental ops (MSLE, LogCosh, Minkowski, Tweedie) use numpy's own log / exp / pow and agree only to a few ulp.
+EXACT_OPS = (0, 1, 2, 3, 4, 8, 9)
+NUM_SUMS = {4: 2, 8: 3, 9: 4, 10: 4}
+
+
+def terms32(op, p, t, param=0.0, eps=0.0):
+    """``[K, ...]`` per-element terms of regression op ``op`` in the kernel's term precision (see above)."""
+    p, t = np.asarray(p), np.asarray(t)
+    f = np.float64 if np.float64 in (p.dtype, t.dtype) else np.float32
+    p, t = p.astype(f), t.astype(f)
+    param, eps, one, two = f(param), f(eps), f(1), f(2)
+    with np.errstate(all="ignore"):
+        if op == 10:  # Tweedie deviance of power `param` + the domain census
+            if param == one:
+                xlogy = np.where(t == 0, f(0), t * np.log(t / p))
+                dev = two * (xlogy + p - t)
+            elif param == two:
+                dev = two * (np.log(p / t) + t / p - one)
+            else:
+                a, b = one - param, two - param
+                dev = two * (np.power(np.fmax(t, f(0)), b) / (a * b) - t * np.power(p, a) / a + np.power(p, b) / b)
+            return np.stack([dev, (p <= 0).astype(f), (t < 0).astype(f), (t == 0).astype(f)])
+        d = p - t
+        if op == 0:
+            out = [d * d]
+        elif op == 1:
+            out = [np.abs(d)]
+        elif op == 2:
+            out = [np.abs(d) / np.fmax(np.abs(t), eps)]
+        elif op == 3:
+            out = [np.abs(d) / np.fmax(np.abs(t) + np.abs(p), eps)]
+        elif op == 4:
+            out = [np.abs(d), np.abs(t)]
+        elif op == 5:
+            lg = np.log1p(p) - np.log1p(t)
+            out = [lg * lg]
+        elif op == 6:
+            out = [np.log((np.exp(d) + np.exp(-d)) / two)]
+        elif op == 7:
+            out = [np.power(np.abs(d), param)]
+        elif op == 8:
+            r = t - p
+            out = [t * t, t, r * r]
+        elif op == 9:
+            r = t - p
+            out = [r, r * r, t, t * t]
+        else:
+            raise ValueError(f"unknown regression op {op}")
+    return np.stack(out)
+
+
+def sums(op, p, t, num_outputs=1, param=0.0, eps=0.0):
+    """``float64 [K, num_outputs]``: the terms of `terms32` summed in float64 over the rows of the ``[n, num_outputs]``
+    row-major view — the layout `_native.regression_sums` returns.  Each output is summed along a contiguous axis, so that
+    numpy's pairwise summation applies (its error grows with log n, not n)."""
+    terms = terms32(op, np.asarray(p).reshape(-1, num_outputs), np.asarray(t).reshape(-1, num_outputs), param, eps)
+    return np.ascontiguousarray(np.moveaxis(terms.astype(np.float64), 1, -1)).sum(-1)
+
 
 def kl_divergence_rows(p, q, log_prob=False):  # kl_divergence.py:25-46 (`_kld_update`), fp64 throughout
     """Per-row KL(p || q).  Probabilities: both rows normalised to sum 1, terms with p = 0 count 0 (`_safe_xlogy`,

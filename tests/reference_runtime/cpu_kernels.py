@@ -243,11 +243,15 @@ _REG_NUM_SUMS = {4: 2, 8: 3, 9: 4}
 
 
 def regression_sums(preds, target, op, num_outputs=1, param=0.0, eps=0.0) -> Tensor:
-    if not preds.is_floating_point():
-        preds = preds.float()
-    target = target.to(preds.dtype)
     d = int(num_outputs)
-    p, t = preds.reshape(-1, d), target.reshape(-1, d)
+    if d < 1 or preds.numel() % d:
+        raise ValueError(f"regression_sums: {preds.numel()} elements do not split into rows of num_outputs={d}")
+    dtype = torch.promote_types(preds.dtype, target.dtype)
+    if not dtype.is_floating_point:
+        dtype = torch.float32
+    if dtype in (torch.float16, torch.bfloat16):  # half-precision inputs: terms in float32 from the upcast values
+        dtype = torch.float32
+    p, t = preds.to(dtype).reshape(-1, d), target.to(dtype).reshape(-1, d)
     diff = p - t
     if op == 0:
         terms = [diff * diff]

@@ -67,3 +67,55 @@ def test_the_other_ops_are_untouched_by_the_shared_header(harness):
     np.testing.assert_allclose(harness(4, 0, 0, "f64", p, t), np.stack([np.abs(d), np.abs(t)], 1))
     np.testing.assert_allclose(harness(8, 0, 0, "f64", p, t), np.stack([t * t, t, (t - p) ** 2], 1))
     np.testing.assert_allclose(harness(9, 0, 0, "f64", p, t), np.stack([t - p, (t - p) ** 2, t, t * t], 1))
+
+
+def _special_pairs(dtype):
+    """Every pair of special values (±0, NaN, ±inf, the extremes and subnormals of `dtype`, small integers) and random
+    values over a wide range of magnitudes, as float64 arrays holding `dtype` values exactly."""
+    fi = np.finfo(dtype)
+    tiny_sub = float(fi.smallest_subnormal)
+    specials = np.array([0.0, -0.0, np.nan, np.inf, -np.inf, float(fi.max), -float(fi.max), float(fi.tiny), -float(fi.tiny),
+                         tiny_sub, -tiny_sub, 3 * tiny_sub, float(fi.tiny) / 3, 1.0, -1.0, 2.0, 0.5, 1e-7, -3.25], dtype=dtype)
+    p, t = np.meshgrid(specials, specials)
+    rng = np.random.default_rng(7)
+    n = 2000
+    rp = (rng.standard_normal(n) * 10.0 ** rng.integers(-30, 30, n)).astype(dtype)
+    rt = (rp.astype(np.float64) * (1 + rng.standard_normal(n) * 10.0 ** rng.integers(-8, 1, n))).astype(dtype)
+    p = np.concatenate([p.ravel(), rp, rng.standard_normal(n).astype(dtype)])
+    t = np.concatenate([t.ravel(), rt, rng.standard_normal(n).astype(dtype)])
+    return p.astype(np.float64), t.astype(np.float64)
+
+
+def _bitwise_equal(a, b):
+    """Equal bit patterns, except that any NaN matches any NaN (the harness prints NaN without its payload)."""
+    both_nan = np.isnan(a) & np.isnan(b)
+    same = a.view(np.uint64) == b.view(np.uint64)
+    return bool(np.all(both_nan | same)), np.flatnonzero(~(both_nan | same))
+
+
+@pytest.mark.parametrize("precision,dtype", [("f32", np.float32), ("f64", np.float64)])
+@pytest.mark.parametrize("op", [0, 1, 2, 3, 4, 8, 9])
+def test_oracle_terms_are_bitwise_the_kernel_term_function(harness, precision, dtype, op):
+    """oracle/regression.py `terms32` against the kernel's own `reg_terms` for the ops made only of IEEE-exact operations:
+    bit for bit, on special, extreme and random values, so that the GPU suite can hold the kernel to exact sums."""
+    from oracle import regression as orr
+
+    p, t = _special_pairs(dtype)
+    for eps in ((1.17e-06, 0.0) if op in (2, 3) else (0.0,)):
+        got = harness(op, 0.0, eps, precision, p, t).T  # [K, n], float64 holding the kernel's term values exactly
+        want = orr.terms32(op, p.astype(dtype), t.astype(dtype), eps=eps).astype(np.float64)
+        assert got.shape == want.shape
+        ok, bad = _bitwise_equal(got, want)
+        assert ok, f"op {op} eps {eps}: first mismatches at p={p[bad[:4] % p.size]}, t={t[bad[:4] % p.size]}"
+
+
+def test_oracle_terms_of_half_inputs_are_the_float32_terms_of_the_upcast_values():
+    from oracle import regression as orr
+
+    rng = np.random.default_rng(3)
+    for half in (np.float16,):
+        p, t = rng.standard_normal(1000).astype(half), rng.standard_normal(1000).astype(half)
+        for op in (0, 3, 9):
+            got = orr.terms32(op, p, t, eps=1.17e-6)
+            assert got.dtype == np.float32
+            np.testing.assert_array_equal(got, orr.terms32(op, p.astype(np.float32), t.astype(np.float32), eps=1.17e-6))
