@@ -135,11 +135,17 @@ CALIBRATION_SIGNATURES = {
     "mb200_calibration_bin_scratch_bytes": ("q", "qq"),
     "mb200_calibration_bin_sums": ("i", "pipiqpqppppqp"),
 }
+# The segmentation overlap-count entry point (K15) is declared in include/metrics_b200_segmentation.h, exported from the same
+# library; tests/test_segmentation_abi.py holds this table to that header.
+SEGMENTATION_SIGNATURES = {
+    "mb200_segmentation_scratch_bytes": ("q", "qqqiiii"),
+    "mb200_segmentation_overlap_counts": ("i", "pipiqqqiiqqiippqpp"),
+}
 
 
 def declare_signatures(handle) -> None:
     """Set ``restype`` / ``argtypes`` of every exported function on a loaded library handle."""
-    for name, (ret, args) in (*SIGNATURES.items(), *CALIBRATION_SIGNATURES.items()):
+    for name, (ret, args) in (*SIGNATURES.items(), *CALIBRATION_SIGNATURES.items(), *SEGMENTATION_SIGNATURES.items()):
         fn = getattr(handle, name)
         fn.restype = _C_TYPES[ret]
         fn.argtypes = [_C_TYPES[a] for a in args]
@@ -959,3 +965,75 @@ def calibration_bin_sums(confidences: Tensor, accuracies: Tensor, boundaries: Te
     if rc:
         check(rc, "calibration_bin_sums")
     return count, sum_conf, sum_acc
+
+
+# ----------------------------------------------------------------------------------------------------------
+# K15 wrapper (segmentation overlap counts, include/metrics_b200_segmentation.h)
+# ----------------------------------------------------------------------------------------------------------
+SEG_PREDS_NEGATIVE, SEG_PREDS_TOO_LARGE, SEG_TARGET_NEGATIVE, SEG_TARGET_TOO_LARGE = 1, 2, 4, 8
+_SEG_FLOAT = (torch.float32, torch.float16, torch.bfloat16)
+
+
+def _dense(strides, shape, step: int) -> bool:
+    """Do these dimensions hold a row-major block whose innermost stride is ``step``?  (Size-1 dimensions never move.)"""
+    for size, stride in zip(reversed(shape), reversed(strides)):
+        if size != 1 and stride != step:
+            return False
+        step *= size
+    return True
+
+
+def _one_hot_layout(x: Tensor) -> Optional[tuple[int, int]]:
+    """(layout, batch stride) when ``x [N, C, ...]`` can be read in place: planar (0: each sample a contiguous ``[C, S]``
+    block) or channels-last (1: each sample a row-major ``[S, C]`` block, what ``one_hot(x).movedim(-1, 1)`` gives); else
+    None."""
+    st, shape = x.stride(), x.shape
+    batch = st[0] if shape[0] > 1 else x[0].numel()
+    if _dense(st[1:], shape[1:], 1):
+        return 0, batch
+    if (shape[1] == 1 or st[1] == 1) and _dense(st[2:], shape[2:], shape[1]):
+        return 1, batch
+    return None
+
+
+def segmentation_overlap_counts(preds: Tensor, target: Tensor, num_classes: int, index_format: bool, mul: bool,
+                                drop_background: bool, err_flag: Optional[Tensor] = None) -> Tensor:
+    """K15 (``mb200_segmentation_overlap_counts``): per-sample, per-class ``(intersection, pred_sum, target_sum)`` as one
+    ``[3, N, C']`` tensor, ``C' = C - 1`` when ``drop_background`` and ``C > 1``.
+
+    Index format: ``preds``, ``target`` int64 labels ``[N, ...]``, ``C = num_classes``; out-of-range labels are left out
+    and OR ``SEG_*`` bits into ``err_flag`` (int32 ``[1]``).  One-hot format: ``[N, C, ...]`` of one dtype, ``C =
+    preds.shape[1]``, read in place when planar or channels-last; the intersection sums ``preds * target`` (``mul``) or
+    ``preds & target`` in the input dtype.  Integer inputs give int64 counts; float inputs give float64 sums (split over
+    many CTAs, folded in a fixed order: deterministic), which the caller rounds to the input dtype.  No host
+    synchronisation."""
+    dev = require_cuda(preds, target)
+    n = preds.shape[0]
+    if index_format:
+        c = int(num_classes)
+        preds = preds.contiguous()
+        target = target.contiguous()
+        inner = preds[0].numel() if n else 0
+        layout, p_sn, t_sn = 0, inner, inner
+    else:
+        c = preds.shape[1]
+        inner = preds[0, 0].numel() if n and c else 0
+        pl, tl = _one_hot_layout(preds), _one_hot_layout(target)
+        if pl is None or tl is None or pl[0] != tl[0]:
+            preds, target = preds.contiguous(), target.contiguous()
+            pl, tl = (0, c * inner), (0, c * inner)
+        layout, p_sn, t_sn = pl[0], pl[1], tl[1]
+    cp = c - 1 if drop_background and c > 1 else c
+    out_dtype = torch.float64 if preds.dtype in _SEG_FLOAT else torch.int64
+    counts = torch.empty((3, n, cp), dtype=out_dtype, device=dev)
+    fmt, drop, lib_ = 0 if index_format else 1, int(bool(drop_background)), lib()
+    nbytes = int(lib_.mb200_segmentation_scratch_bytes(n, c, inner, fmt, layout, tag(preds), drop))
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev) if nbytes > 0 else None
+    with on_device(dev):
+        rc = lib_.mb200_segmentation_overlap_counts(
+            preds.data_ptr(), tag(preds), target.data_ptr(), tag(target), n, c, inner, fmt, layout, p_sn, t_sn,
+            int(bool(mul)), drop, counts.data_ptr(), ptr(scratch), max(nbytes, 0), ptr(err_flag), stream_handle(dev),
+        )
+    if rc:
+        check(rc, "segmentation_overlap_counts")
+    return counts
