@@ -404,8 +404,8 @@ static int binary_stat_counts_impl(const void* preds, int preds_dtype, const voi
     const long long total = n_outer * num_labels * inner;
     if (total == 0) return 0;
     MB200_REQUIRE(preds && target && counts, "NULL pointer");
-    MB200_REQUIRE(target_dtype >= MB200_I64 && target_dtype <= MB200_BOOL, "target must be an integer tensor");
-    const bool float_preds = preds_dtype <= MB200_F64;
+    MB200_REQUIRE(is_label_tag(target_dtype), "target must be an integer tensor");
+    const bool float_preds = is_float_tag(preds_dtype);
     MB200_REQUIRE(!float_preds || flag_scratch, "flag_scratch is required for floating scores");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const long long groups = samplewise ? n_outer * num_labels : num_labels;
@@ -444,11 +444,10 @@ static int binary_stat_counts_impl(const void* preds, int preds_dtype, const voi
         } else {
             b.x_lo = b.x_hi = std::nanf("");
         }
-        switch (preds_dtype) {
-            case MB200_F32: bin_count_flat_both_kernel<float><<<grid, 256, 0, st>>>(a, b); break;
-            case MB200_F16: bin_count_flat_both_kernel<__half><<<grid, 256, 0, st>>>(a, b); break;
-            default: bin_count_flat_both_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(a, b); break;
-        }
+        with_float_type<kNoF64>(preds_dtype, [&](auto t) {
+            bin_count_flat_both_kernel<typename decltype(t)::type><<<grid, 256, 0, st>>>(a, b);
+            return 0;
+        });
         bin_select_kernel<<<1, 32, 0, st>>>(b.both, b.vote, a.counts);
         count_launch();
         count_launch();
@@ -457,41 +456,34 @@ static int binary_stat_counts_impl(const void* preds, int preds_dtype, const voi
     if (float_preds) {
         MB200_CUDA_OK(cudaMemsetAsync(flag_scratch, 0, sizeof(uint32_t), st));
         const int fgrid = (int)std::min<long long>(cap, (total + 2047) / 2048);
-        switch (preds_dtype) {
-            case MB200_F32: bin_range_flag_kernel<float><<<fgrid, 256, 0, st>>>((const float*)preds, total, flag_scratch); break;
-            case MB200_F16: bin_range_flag_kernel<__half><<<fgrid, 256, 0, st>>>((const __half*)preds, total, flag_scratch); break;
-            case MB200_BF16: bin_range_flag_kernel<__nv_bfloat16><<<fgrid, 256, 0, st>>>((const __nv_bfloat16*)preds, total, flag_scratch); break;
-            case MB200_F64: bin_range_flag_kernel<double><<<fgrid, 256, 0, st>>>((const double*)preds, total, flag_scratch); break;
-        }
+        with_float_type(preds_dtype, [&](auto t) {
+            using T = typename decltype(t)::type;
+            bin_range_flag_kernel<T><<<fgrid, 256, 0, st>>>((const T*)preds, total, flag_scratch);
+            return 0;
+        });
         count_launch();
     }
     if (flat) {
-        switch (preds_dtype) {
-            case MB200_F32: bin_count_flat_kernel<float><<<grid, 256, 0, st>>>(a); break;
-            case MB200_F16: bin_count_flat_kernel<__half><<<grid, 256, 0, st>>>(a); break;
-            case MB200_BF16: bin_count_flat_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(a); break;
-            default: bin_count_flat_kernel<double><<<grid, 256, 0, st>>>(a); break;
-        }
+        with_float_type(preds_dtype, [&](auto t) {
+            bin_count_flat_kernel<typename decltype(t)::type><<<grid, 256, 0, st>>>(a);
+            return 0;
+        });
         count_launch();
         return check_cuda(cudaGetLastError(), "binary stat counts launch");
     }
     if (float_preds && !samplewise && inner == 1 && num_labels >= 2 && num_labels <= 256) {
-        switch (preds_dtype) {
-            case MB200_F32: bin_count_cols_kernel<float><<<grid, 256, 0, st>>>(a); break;
-            case MB200_F16: bin_count_cols_kernel<__half><<<grid, 256, 0, st>>>(a); break;
-            case MB200_BF16: bin_count_cols_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(a); break;
-            default: bin_count_cols_kernel<double><<<grid, 256, 0, st>>>(a); break;
-        }
+        with_float_type(preds_dtype, [&](auto t) {
+            bin_count_cols_kernel<typename decltype(t)::type><<<grid, 256, 0, st>>>(a);
+            return 0;
+        });
         count_launch();
         return check_cuda(cudaGetLastError(), "binary stat counts launch");
     }
-    switch (preds_dtype) {
-        case MB200_F32: bin_count_kernel<float><<<grid, 256, smem, st>>>(a); break;
-        case MB200_F16: bin_count_kernel<__half><<<grid, 256, smem, st>>>(a); break;
-        case MB200_BF16: bin_count_kernel<__nv_bfloat16><<<grid, 256, smem, st>>>(a); break;
-        case MB200_F64: bin_count_kernel<double><<<grid, 256, smem, st>>>(a); break;
-        default: bin_count_kernel<IntPred><<<grid, 256, smem, st>>>(a); break;
-    }
+    const int rc = with_float_type(preds_dtype, [&](auto t) {
+        bin_count_kernel<typename decltype(t)::type><<<grid, 256, smem, st>>>(a);
+        return 0;
+    });
+    if (rc == kNoType) bin_count_kernel<IntPred><<<grid, 256, smem, st>>>(a);
     count_launch();
     return check_cuda(cudaGetLastError(), "binary stat counts launch");
 }

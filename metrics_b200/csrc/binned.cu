@@ -310,6 +310,7 @@ static int binned_update_impl(int multilabel, const void* preds, int preds_dtype
     MB200_REQUIRE(num_thresholds < (1 << 24) && num_classes < (1 << 24), "sizes too large");
     if (n == 0) return 0;
     MB200_REQUIRE(preds && target && thresholds_sorted && confmat && scratch, "NULL pointer");
+    MB200_REQUIRE(is_float_tag(preds_dtype), "scores must be floating point (dtype tag %d)", preds_dtype);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const long long total = n * num_classes;
     const size_t smem_need = (size_t)num_classes * 2 * (num_thresholds + 1) * sizeof(unsigned);
@@ -349,18 +350,13 @@ static int binned_update_impl(int multilabel, const void* preds, int preds_dtype
         count_launch();
         return check_cuda(cudaGetLastError(), "binned curve launch");
     }
-#define MB200_BINNED(T)                                                                                              \
-    binned_bucket_kernel<T><<<(int)blocks, 256, smem_total, st>>>(                                                  \
-        reinterpret_cast<const T*>(preds), target, target_dtype, n, (int)num_classes, thresholds_sorted,            \
-        (int)num_thresholds, sc, cm, use_smem, multilabel, thr_in_smem);
-    switch (preds_dtype) {
-        case MB200_F32: MB200_BINNED(float) break;
-        case MB200_F16: MB200_BINNED(__half) break;
-        case MB200_BF16: MB200_BINNED(__nv_bfloat16) break;
-        case MB200_F64: MB200_BINNED(double) break;
-        default: set_error("scores must be floating point (dtype tag %d)", preds_dtype); return MB200_ERR_INVALID;
-    }
-#undef MB200_BINNED
+    with_float_type(preds_dtype, [&](auto t) {
+        using T = typename decltype(t)::type;
+        binned_bucket_kernel<T><<<(int)blocks, 256, smem_total, st>>>(reinterpret_cast<const T*>(preds), target, target_dtype, n,
+                                                                     (int)num_classes, thresholds_sorted, (int)num_thresholds, sc,
+                                                                     cm, use_smem, multilabel, thr_in_smem);
+        return 0;
+    });
     count_launch();
     return check_cuda(cudaGetLastError(), "binned curve launch");
 }

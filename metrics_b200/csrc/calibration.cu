@@ -487,9 +487,6 @@ int launch_bin_sums(const void* confidences, const void* accuracies, int acc_dty
     return check_cuda(cudaGetLastError(), "calibration binning launch");
 }
 
-bool is_float_tag(int d) { return d == MB200_F32 || d == MB200_F16 || d == MB200_BF16 || d == MB200_F64; }
-bool is_label_tag(int d) { return d >= MB200_I64 && d <= MB200_BOOL; }
-
 }  // namespace
 }  // namespace mb200
 
@@ -518,12 +515,10 @@ extern "C" int mb200_calibration_top_label(const void* preds, int preds_dtype, c
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     unsigned char* s = reinterpret_cast<unsigned char*>(scratch);
     const int N = (int)n, C = (int)num_classes;
-    switch (preds_dtype) {
-        case MB200_F32: return launch_top_label<float>(preds, target, target_dtype, N, C, has_ignore, ignore_index, confidence, accuracy, s, err_flag, st);
-        case MB200_F16: return launch_top_label<__half>(preds, target, target_dtype, N, C, has_ignore, ignore_index, confidence, accuracy, s, err_flag, st);
-        case MB200_BF16: return launch_top_label<__nv_bfloat16>(preds, target, target_dtype, N, C, has_ignore, ignore_index, confidence, accuracy, s, err_flag, st);
-        default: return launch_top_label<double>(preds, target, target_dtype, N, C, has_ignore, ignore_index, confidence, accuracy, s, err_flag, st);
-    }
+    return with_float_type(preds_dtype, [&](auto t) {
+        return launch_top_label<typename decltype(t)::type>(preds, target, target_dtype, N, C, has_ignore, ignore_index, confidence,
+                                                            accuracy, s, err_flag, st);
+    });
 }
 
 extern "C" int64_t mb200_calibration_bin_scratch_bytes(int64_t n, int64_t n_bins) {
@@ -546,10 +541,8 @@ extern "C" int mb200_calibration_bin_sums(const void* confidences, int conf_dtyp
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int slots = (int)(n_bins + 1);
     double* part = reinterpret_cast<double*>(scratch);
-    switch (conf_dtype) {
-        case MB200_F32: return launch_bin_sums<float>(confidences, accuracies, acc_dtype, n, boundaries, slots, count, sum_conf, sum_acc, part, st);
-        case MB200_F16: return launch_bin_sums<__half>(confidences, accuracies, acc_dtype, n, boundaries, slots, count, sum_conf, sum_acc, part, st);
-        case MB200_BF16: return launch_bin_sums<__nv_bfloat16>(confidences, accuracies, acc_dtype, n, boundaries, slots, count, sum_conf, sum_acc, part, st);
-        default: return launch_bin_sums<double>(confidences, accuracies, acc_dtype, n, boundaries, slots, count, sum_conf, sum_acc, part, st);
-    }
+    return with_float_type(conf_dtype, [&](auto t) {
+        return launch_bin_sums<typename decltype(t)::type>(confidences, accuracies, acc_dtype, n, boundaries, slots, count, sum_conf,
+                                                           sum_acc, part, st);
+    });
 }

@@ -5,9 +5,11 @@
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <limits.h>
 #include <stdint.h>
 #include <stdio.h>
 
+#include <type_traits>
 #include <unordered_map>
 
 #include "../../include/metrics_b200.h"
@@ -35,6 +37,39 @@ int sm_count();  // cached multiprocessor count of the current device
             return MB200_ERR_INVALID;                            \
         }                                                        \
     } while (0)
+
+// ---- dtype tags (enum mb200_dtype) -----------------------------------------------------------------
+// An entry point checks its score tag with is_float_tag before its first CUDA call, under its own error code and message,
+// then picks the kernel instantiation with with_float_type.  kNoF64 selects the score types of kernels without an f64
+// instantiation: f32 / f16 / bf16.
+constexpr bool kNoF64 = false;
+
+template <bool kF64 = true>
+constexpr bool is_float_tag(int d) {
+    return d == MB200_F32 || d == MB200_F16 || d == MB200_BF16 || (kF64 && d == MB200_F64);
+}
+constexpr bool is_label_tag(int d) { return d >= MB200_I64 && d <= MB200_BOOL; }
+
+template <typename T>
+struct As {
+    using type = T;
+};
+constexpr int kNoType = INT_MIN;
+
+// Returns f(As<T>{}) for the score type T of `dtype`: float, __half, __nv_bfloat16, and double unless kF64 is false.
+// Any tag for which is_float_tag<kF64> is false returns kNoType without calling f.
+template <bool kF64 = true, typename F>
+int with_float_type(int dtype, F&& f) {
+    switch (dtype) {
+        case MB200_F32: return f(As<float>{});
+        case MB200_F16: return f(As<__half>{});
+        case MB200_BF16: return f(As<__nv_bfloat16>{});
+        case MB200_F64:
+            if constexpr (kF64) return f(As<double>{});
+            return kNoType;
+        default: return kNoType;
+    }
+}
 
 // ---- device helpers -------------------------------------------------------------------------------
 // Streaming 16-byte load: data is consumed exactly once, keep it out of L1.

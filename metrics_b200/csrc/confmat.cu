@@ -449,8 +449,8 @@ static int dispatch_rows_t(int preds_dtype, int preds_has_class_dim, const RowAr
                            cudaStream_t st) {
     if (!preds_has_class_dim) {
         if constexpr (Sink::kNeedsTarget) {
-            MB200_REQUIRE(preds_dtype >= MB200_I64 && preds_dtype <= MB200_BOOL,
-                          "label-format preds must have an integer dtype (got dtype tag %d)", preds_dtype);
+            MB200_REQUIRE(is_label_tag(preds_dtype), "label-format preds must have an integer dtype (got dtype tag %d)",
+                          preds_dtype);
             auto kern = labels_kernel<Sink, kI64>;
             const int grid = grid_for(a.n_outer * a.inner, kRowThreads, resident_blocks(kern, kRowThreads, smem));
             kern<<<grid, kRowThreads, smem, st>>>(a, preds_dtype, sink);
@@ -461,15 +461,10 @@ static int dispatch_rows_t(int preds_dtype, int preds_has_class_dim, const RowAr
             return MB200_ERR_INVALID;
         }
     }
-    switch (preds_dtype) {
-        case MB200_BF16: return launch_rows<__nv_bfloat16, Sink, kI64>(a, sink, smem, st);
-        case MB200_F16: return launch_rows<__half, Sink, kI64>(a, sink, smem, st);
-        case MB200_F32: return launch_rows<float, Sink, kI64>(a, sink, smem, st);
-        case MB200_F64: return launch_rows<double, Sink, kI64>(a, sink, smem, st);
-        default:
-            set_error("preds with a class dimension must be floating point (got dtype tag %d)", preds_dtype);
-            return MB200_ERR_INVALID;
-    }
+    MB200_REQUIRE(is_float_tag(preds_dtype), "preds with a class dimension must be floating point (got dtype tag %d)",
+                  preds_dtype);
+    return with_float_type(preds_dtype,
+                           [&](auto t) { return launch_rows<typename decltype(t)::type, Sink, kI64>(a, sink, smem, st); });
 }
 
 template <typename Sink>
@@ -492,8 +487,7 @@ static int validate_common(const void* preds, const void* target, int target_dty
         if (need_target) MB200_REQUIRE(target != nullptr, "target is NULL");
     }
     if (need_target)
-        MB200_REQUIRE(target_dtype >= MB200_I64 && target_dtype <= MB200_BOOL,
-                      "target must have an integer dtype (got dtype tag %d)", target_dtype);
+        MB200_REQUIRE(is_label_tag(target_dtype), "target must have an integer dtype (got dtype tag %d)", target_dtype);
     return 0;
 }
 
@@ -564,20 +558,13 @@ extern "C" int mb200_multiclass_stat_scores_update(const void* preds, int preds_
 
 template <typename Sink, bool kI64>
 static int launch_topk_t(int preds_dtype, const RowArgs& a, Sink sink, size_t smem, int top_k, cudaStream_t st) {
-#define MB200_TOPK(T)                                                                                        \
-    {                                                                                                        \
-        auto kern = rows_topk_kernel<T, Sink, kI64>;                                                         \
-        const int grid = grid_for(a.n_outer, kRowThreads / 32, resident_blocks(kern, kRowThreads, smem));   \
-        kern<<<grid, kRowThreads, smem, st>>>(a, sink, top_k);                                               \
-    }
-    switch (preds_dtype) {
-        case MB200_BF16: MB200_TOPK(__nv_bfloat16) break;
-        case MB200_F16: MB200_TOPK(__half) break;
-        case MB200_F32: MB200_TOPK(float) break;
-        case MB200_F64: MB200_TOPK(double) break;
-        default: set_error("top-k needs floating scores (dtype tag %d)", preds_dtype); return MB200_ERR_INVALID;
-    }
-#undef MB200_TOPK
+    MB200_REQUIRE(is_float_tag(preds_dtype), "top-k needs floating scores (dtype tag %d)", preds_dtype);
+    with_float_type(preds_dtype, [&](auto t) {
+        auto kern = rows_topk_kernel<typename decltype(t)::type, Sink, kI64>;
+        const int grid = grid_for(a.n_outer, kRowThreads / 32, resident_blocks(kern, kRowThreads, smem));
+        kern<<<grid, kRowThreads, smem, st>>>(a, sink, top_k);
+        return 0;
+    });
     count_launch();
     return check_cuda(cudaGetLastError(), "top-k kernel launch");
 }

@@ -1014,35 +1014,24 @@ extern "C" int mb200_curve_sigmoid_if_logits(const void* preds, int dtype, int64
     MB200_REQUIRE(n >= 0, "negative n");
     if (n == 0) return 0;
     MB200_REQUIRE(preds && out && flag_scratch, "NULL pointer");
+    MB200_REQUIRE(is_float_tag(dtype), "scores must be floating point (dtype tag %d)", dtype);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    if (n <= 1024 * (dtype == MB200_F64 ? kSmallItemsF64 : kSmallItems)) {
-        switch (dtype) {
-            case MB200_F32: sigmoid_if_small_kernel<float, kSmallItems><<<1, 1024, 0, st>>>((const float*)preds, (float*)out, (int)n); break;
-            case MB200_F16: sigmoid_if_small_kernel<__half, kSmallItems><<<1, 1024, 0, st>>>((const __half*)preds, (__half*)out, (int)n); break;
-            case MB200_BF16: sigmoid_if_small_kernel<__nv_bfloat16, kSmallItems><<<1, 1024, 0, st>>>((const __nv_bfloat16*)preds, (__nv_bfloat16*)out, (int)n); break;
-            case MB200_F64: sigmoid_if_small_kernel<double, kSmallItemsF64><<<1, 1024, 0, st>>>((const double*)preds, (double*)out, (int)n); break;
-            default: set_error("scores must be floating point (dtype tag %d)", dtype); return MB200_ERR_INVALID;
+    return with_float_type(dtype, [&](auto t) {
+        using T = typename decltype(t)::type;
+        constexpr int kItems = std::is_same_v<T, double> ? kSmallItemsF64 : kSmallItems;
+        if (n <= 1024 * kItems) {
+            sigmoid_if_small_kernel<T, kItems><<<1, 1024, 0, st>>>((const T*)preds, (T*)out, (int)n);
+            count_launch();
+            return check_cuda(cudaGetLastError(), "curve format launch");
         }
+        MB200_CUDA_OK(cudaMemsetAsync(flag_scratch, 0, sizeof(uint32_t), st));
+        const int grid = blocks_for(n, 256 * 8, sm_count() * 8);
+        range_flag_kernel<T><<<grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), n, flag_scratch);
+        sigmoid_if_kernel<T><<<grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), reinterpret_cast<T*>(out), n, flag_scratch);
+        count_launch();
         count_launch();
         return check_cuda(cudaGetLastError(), "curve format launch");
-    }
-    MB200_CUDA_OK(cudaMemsetAsync(flag_scratch, 0, sizeof(uint32_t), st));
-    const int grid = blocks_for(n, 256 * 8, sm_count() * 8);
-#define MB200_FMT(T)                                                                                             \
-    range_flag_kernel<T><<<grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), n, flag_scratch);             \
-    sigmoid_if_kernel<T><<<grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), reinterpret_cast<T*>(out), n, \
-                                               flag_scratch);
-    switch (dtype) {
-        case MB200_F32: MB200_FMT(float) break;
-        case MB200_F16: MB200_FMT(__half) break;
-        case MB200_BF16: MB200_FMT(__nv_bfloat16) break;
-        case MB200_F64: MB200_FMT(double) break;
-        default: set_error("scores must be floating point (dtype tag %d)", dtype); return MB200_ERR_INVALID;
-    }
-#undef MB200_FMT
-    count_launch();
-    count_launch();
-    return check_cuda(cudaGetLastError(), "curve format launch");
+    });
 }
 
 extern "C" int mb200_curve_softmax_if_logits(const void* preds, int dtype, int64_t n, int64_t num_classes, void* out,
@@ -1051,23 +1040,19 @@ extern "C" int mb200_curve_softmax_if_logits(const void* preds, int dtype, int64
     if (n == 0) return 0;
     MB200_REQUIRE(preds && out && flag_scratch, "NULL pointer");
     MB200_REQUIRE(n < (1ll << 31) && num_classes < (1ll << 31), "sizes exceed int32");
+    MB200_REQUIRE(is_float_tag(dtype), "softmax scores must be f32/f16/bf16/f64 (dtype tag %d)", dtype);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     MB200_CUDA_OK(cudaMemsetAsync(flag_scratch, 0, sizeof(uint32_t), st));
     const long long total = n * num_classes;
     const int grid = blocks_for(total, 256 * 8, sm_count() * 8);
     const int grid_rows = blocks_for(n, 8, sm_count() * 8);
-#define MB200_FMT(T)                                                                                                \
-    range_flag_kernel<T><<<grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), total, flag_scratch);            \
-    softmax_if_kernel<T><<<grid_rows, 256, 0, st>>>(reinterpret_cast<const T*>(preds), reinterpret_cast<T*>(out),  \
-                                                    (int)n, (int)num_classes, flag_scratch);
-    switch (dtype) {
-        case MB200_F32: MB200_FMT(float) break;
-        case MB200_F16: MB200_FMT(__half) break;
-        case MB200_BF16: MB200_FMT(__nv_bfloat16) break;
-        case MB200_F64: MB200_FMT(double) break;
-        default: set_error("softmax scores must be f32/f16/bf16/f64 (dtype tag %d)", dtype); return MB200_ERR_INVALID;
-    }
-#undef MB200_FMT
+    with_float_type(dtype, [&](auto t) {
+        using T = typename decltype(t)::type;
+        range_flag_kernel<T><<<grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), total, flag_scratch);
+        softmax_if_kernel<T><<<grid_rows, 256, 0, st>>>(reinterpret_cast<const T*>(preds), reinterpret_cast<T*>(out), (int)n,
+                                                        (int)num_classes, flag_scratch);
+        return 0;
+    });
     count_launch();
     count_launch();
     return check_cuda(cudaGetLastError(), "curve softmax launch");
@@ -1260,18 +1245,15 @@ static int curve_evaluate_impl(const void* preds, int preds_dtype, const void* t
     MB200_REQUIRE((fps_out == nullptr) == (tps_out == nullptr) && (fps_out == nullptr) == (thr_out == nullptr),
                   "curve outputs must be given all together or not at all");
     MB200_REQUIRE(segments <= 65535, "at most 65535 curves per call");
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-#define MB200_EVAL(T)                                                                                                  \
-    return evaluate_typed<T>(preds, target, target_dtype, n, segments, pos_label, workspace, out_auroc, out_ap, out_counts, \
-                             fps_out, tps_out, thr_out, err_flag, st, unit_range)
-    switch (preds_dtype) {
-        case MB200_F32: MB200_EVAL(float);
-        case MB200_F16: MB200_EVAL(__half);
-        case MB200_BF16: MB200_EVAL(__nv_bfloat16);
-        case MB200_F64: MB200_EVAL(double);
-        default: set_error("scores must be f32/f16/bf16/f64 (dtype tag %d)", preds_dtype); return MB200_ERR_UNSUPPORTED;
+    if (!is_float_tag(preds_dtype)) {
+        set_error("scores must be f32/f16/bf16/f64 (dtype tag %d)", preds_dtype);
+        return MB200_ERR_UNSUPPORTED;
     }
-#undef MB200_EVAL
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    return with_float_type(preds_dtype, [&](auto t) {
+        return evaluate_typed<typename decltype(t)::type>(preds, target, target_dtype, n, segments, pos_label, workspace, out_auroc,
+                                                          out_ap, out_counts, fps_out, tps_out, thr_out, err_flag, st, unit_range);
+    });
 }
 
 extern "C" int mb200_curve_evaluate(const void* preds, int preds_dtype, const void* target, int target_dtype,
@@ -1308,18 +1290,16 @@ extern "C" int mb200_curve_evaluate_multilabel(const void* preds, int preds_dtyp
     MB200_REQUIRE(workspace_bytes >= mb200_curve_workspace_bytes_for(num_labels, n, preds_dtype), "workspace too small");
     MB200_REQUIRE((fps_out == nullptr) == (tps_out == nullptr) && (fps_out == nullptr) == (thr_out == nullptr),
                   "curve outputs must be given all together or not at all");
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-#define MB200_EVAL(T)                                                                                                   \
-    return evaluate_multilabel_typed<T>(preds, target, target_dtype, n, num_labels, has_ignore, ignore_index, workspace, \
-                                        out_auroc, out_ap, out_counts, fps_out, tps_out, thr_out, err_flag, st)
-    switch (preds_dtype) {
-        case MB200_F32: MB200_EVAL(float);
-        case MB200_F16: MB200_EVAL(__half);
-        case MB200_BF16: MB200_EVAL(__nv_bfloat16);
-        case MB200_F64: MB200_EVAL(double);
-        default: set_error("scores must be f32/f16/bf16/f64 (dtype tag %d)", preds_dtype); return MB200_ERR_UNSUPPORTED;
+    if (!is_float_tag(preds_dtype)) {
+        set_error("scores must be f32/f16/bf16/f64 (dtype tag %d)", preds_dtype);
+        return MB200_ERR_UNSUPPORTED;
     }
-#undef MB200_EVAL
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    return with_float_type(preds_dtype, [&](auto t) {
+        return evaluate_multilabel_typed<typename decltype(t)::type>(preds, target, target_dtype, n, num_labels, has_ignore,
+                                                                     ignore_index, workspace, out_auroc, out_ap, out_counts,
+                                                                     fps_out, tps_out, thr_out, err_flag, st);
+    });
 }
 
 // Class-major keys of [n, num_classes] scores: keys_out [num_classes][n] (the packing step of mb200_curve_evaluate on
@@ -1329,14 +1309,17 @@ extern "C" int mb200_curve_pack_keys(const void* preds, int preds_dtype, int64_t
     MB200_REQUIRE(n >= 0 && num_classes >= 1 && n < (1ll << 30), "bad sizes");
     if (n == 0) return 0;
     MB200_REQUIRE(preds && keys_out, "NULL pointer");
+    if (!is_float_tag<kNoF64>(preds_dtype)) {
+        set_error("scores must be f32/f16/bf16 (dtype tag %d)", preds_dtype);
+        return MB200_ERR_UNSUPPORTED;
+    }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const dim3 grid((unsigned)((n + 31) / 32), (unsigned)((num_classes + 31) / 32));
-    switch (preds_dtype) {
-        case MB200_F32: pack_keys_kernel<float><<<grid, 256, 0, st>>>((const float*)preds, (int)n, (int)num_classes, keys_out); break;
-        case MB200_F16: pack_keys_kernel<__half><<<grid, 256, 0, st>>>((const __half*)preds, (int)n, (int)num_classes, keys_out); break;
-        case MB200_BF16: pack_keys_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>((const __nv_bfloat16*)preds, (int)n, (int)num_classes, keys_out); break;
-        default: set_error("scores must be f32/f16/bf16 (dtype tag %d)", preds_dtype); return MB200_ERR_UNSUPPORTED;
-    }
+    with_float_type<kNoF64>(preds_dtype, [&](auto t) {
+        using T = typename decltype(t)::type;
+        pack_keys_kernel<T><<<grid, 256, 0, st>>>((const T*)preds, (int)n, (int)num_classes, keys_out);
+        return 0;
+    });
     count_launch();
     return check_cuda(cudaGetLastError(), "curve pack keys launch");
 }
@@ -1419,18 +1402,15 @@ extern "C" int mb200_curve_weighted_clf_curve(const void* preds, int preds_dtype
     MB200_REQUIRE(n >= 1 && n < (1ll << 30), "curve evaluation needs 1 <= n < 2^30 samples (got %lld)", (long long)n);
     MB200_REQUIRE(preds && target && weights && workspace && fps_out && tps_out && thr_out && count_out, "NULL pointer");
     MB200_REQUIRE(workspace_bytes >= mb200_curve_weighted_workspace_bytes(n, preds_dtype), "workspace too small");
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-#define MB200_W(T)                                                                                                       \
-    return weighted_typed<T>(preds, target, target_dtype, weights, n, pos_label, workspace, fps_out, tps_out, thr_out,  \
-                             count_out, err_flag, st)
-    switch (preds_dtype) {
-        case MB200_F32: MB200_W(float);
-        case MB200_F16: MB200_W(__half);
-        case MB200_BF16: MB200_W(__nv_bfloat16);
-        case MB200_F64: MB200_W(double);
-        default: set_error("scores must be f32/f16/bf16/f64 (dtype tag %d)", preds_dtype); return MB200_ERR_UNSUPPORTED;
+    if (!is_float_tag(preds_dtype)) {
+        set_error("scores must be f32/f16/bf16/f64 (dtype tag %d)", preds_dtype);
+        return MB200_ERR_UNSUPPORTED;
     }
-#undef MB200_W
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    return with_float_type(preds_dtype, [&](auto t) {
+        return weighted_typed<typename decltype(t)::type>(preds, target, target_dtype, weights, n, pos_label, workspace, fps_out,
+                                                          tps_out, thr_out, count_out, err_flag, st);
+    });
 }
 
 extern "C" int64_t mb200_curve_normalize_scratch_bytes(int64_t n) {
@@ -1450,6 +1430,7 @@ extern "C" int mb200_curve_sigmoid_if_logits_scratch(const void* preds, int dtyp
                       ((reinterpret_cast<uintptr_t>(preds) | reinterpret_cast<uintptr_t>(out)) & 15) == 0 &&
                       (reinterpret_cast<uintptr_t>(scratch) & 3) == 0;
     if (!spec) return mb200_curve_sigmoid_if_logits(preds, dtype, n, out, reinterpret_cast<uint32_t*>(scratch), stream);
+    MB200_REQUIRE(is_float_tag<kNoF64>(dtype), "scores must be floating point (dtype tag %d)", dtype);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int esize = dtype == MB200_F32 ? 4 : 2;
     const long long kvec = 16 / esize;
@@ -1461,18 +1442,14 @@ extern "C" int mb200_curve_sigmoid_if_logits_scratch(const void* preds, int dtyp
     long long grid = ntiles;
     const long long cap = (long long)sm_count() * 8;
     if (grid > cap) grid = cap;
-#define MB200_SPEC(T)                                                                                                         \
-    sigmoid_spec_kernel<T, false><<<(unsigned)grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), reinterpret_cast<T*>(out), n, \
-                                                                 vote, pending, ntiles);                                      \
-    sigmoid_spec_kernel<T, true><<<(unsigned)grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), reinterpret_cast<T*>(out), n,  \
-                                                                vote, pending, ntiles);
-    switch (dtype) {
-        case MB200_F32: MB200_SPEC(float) break;
-        case MB200_F16: MB200_SPEC(__half) break;
-        case MB200_BF16: MB200_SPEC(__nv_bfloat16) break;
-        default: set_error("scores must be floating point (dtype tag %d)", dtype); return MB200_ERR_INVALID;
-    }
-#undef MB200_SPEC
+    with_float_type<kNoF64>(dtype, [&](auto t) {
+        using T = typename decltype(t)::type;
+        sigmoid_spec_kernel<T, false><<<(unsigned)grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), reinterpret_cast<T*>(out),
+                                                                     n, vote, pending, ntiles);
+        sigmoid_spec_kernel<T, true><<<(unsigned)grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), reinterpret_cast<T*>(out),
+                                                                    n, vote, pending, ntiles);
+        return 0;
+    });
     count_launch();
     count_launch();
     return check_cuda(cudaGetLastError(), "curve format launch");
@@ -1489,32 +1466,30 @@ extern "C" int mb200_curve_softmax_if_logits_scratch(const void* preds, int dtyp
     const bool spec = dtype != MB200_F64 && num_classes <= 1024 && scratch_bytes >= 8 + n &&
                       (reinterpret_cast<uintptr_t>(scratch) & 3) == 0;
     if (!spec) return mb200_curve_softmax_if_logits(preds, dtype, n, num_classes, out, reinterpret_cast<uint32_t*>(scratch), stream);
+    MB200_REQUIRE(is_float_tag<kNoF64>(dtype), "softmax scores must be f32/f16/bf16/f64 (dtype tag %d)", dtype);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     MB200_CUDA_OK(cudaMemsetAsync(scratch, 0, (size_t)(8 + n), st));
     unsigned* vote = reinterpret_cast<unsigned*>(scratch);
     unsigned char* pending = reinterpret_cast<unsigned char*>(scratch) + 8;
     const int grid = blocks_for(n, 8, sm_count() * 3);  // 3 resident CTAs per SM (<= 85 registers): one wave
     const int C = (int)num_classes;
-#define MB200_SMX2(T, ITER)                                                                                                  \
-    softmax_spec_kernel<T, ITER, false><<<grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), reinterpret_cast<T*>(out),   \
-                                                              (int)n, C, vote, pending);                                     \
-    softmax_spec_kernel<T, ITER, true><<<grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), reinterpret_cast<T*>(out),    \
-                                                             (int)n, C, vote, pending);
-#define MB200_SMX(T)                       \
-    if (C <= 32) { MB200_SMX2(T, 1) }       \
-    else if (C <= 64) { MB200_SMX2(T, 2) }  \
-    else if (C <= 128) { MB200_SMX2(T, 4) } \
-    else if (C <= 256) { MB200_SMX2(T, 8) } \
-    else if (C <= 512) { MB200_SMX2(T, 16) } \
-    else { MB200_SMX2(T, 32) }
-    switch (dtype) {
-        case MB200_F32: MB200_SMX(float) break;
-        case MB200_F16: MB200_SMX(__half) break;
-        case MB200_BF16: MB200_SMX(__nv_bfloat16) break;
-        default: set_error("softmax scores must be f32/f16/bf16/f64 (dtype tag %d)", dtype); return MB200_ERR_INVALID;
-    }
-#undef MB200_SMX
-#undef MB200_SMX2
+    with_float_type<kNoF64>(dtype, [&](auto t) {
+        using T = typename decltype(t)::type;
+        const auto launch = [&](auto iter) {
+            constexpr int kIter = decltype(iter)::value;
+            softmax_spec_kernel<T, kIter, false><<<grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), reinterpret_cast<T*>(out),
+                                                                       (int)n, C, vote, pending);
+            softmax_spec_kernel<T, kIter, true><<<grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), reinterpret_cast<T*>(out),
+                                                                      (int)n, C, vote, pending);
+        };
+        if (C <= 32) launch(std::integral_constant<int, 1>{});
+        else if (C <= 64) launch(std::integral_constant<int, 2>{});
+        else if (C <= 128) launch(std::integral_constant<int, 4>{});
+        else if (C <= 256) launch(std::integral_constant<int, 8>{});
+        else if (C <= 512) launch(std::integral_constant<int, 16>{});
+        else launch(std::integral_constant<int, 32>{});
+        return 0;
+    });
     count_launch();
     count_launch();
     return check_cuda(cudaGetLastError(), "curve softmax launch");

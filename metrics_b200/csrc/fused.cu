@@ -154,23 +154,18 @@ extern "C" int mb200_multiclass_stats_softmax_update(const void* preds, int pred
     MB200_REQUIRE(num_classes >= 1 && num_classes <= 1024, "the fused update keeps a row in registers: 1 <= num_classes <= 1024 (got %lld)",
                   (long long)num_classes);
     MB200_REQUIRE(tp && fp && tn && fn && workspace && logits_flag, "state / workspace / flag pointer is NULL");
-    MB200_REQUIRE(target_dtype >= MB200_I64 && target_dtype <= MB200_BOOL, "target must have an integer dtype (got dtype tag %d)",
-                  target_dtype);
+    MB200_REQUIRE(is_label_tag(target_dtype), "target must have an integer dtype (got dtype tag %d)", target_dtype);
     if (n == 0) return 0;
     MB200_REQUIRE(preds && target && probs_out, "NULL pointer");
+    MB200_REQUIRE(is_float_tag<kNoF64>(preds_dtype), "scores must be f32/f16/bf16 (dtype tag %d)", preds_dtype);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     MB200_CUDA_OK(cudaMemsetAsync(logits_flag, 0, sizeof(uint32_t), st));
     StatsSink<false> sink{(long long*)tp, (long long*)fp, (long long*)tn, (long long*)fn, (long long*)workspace,
                           (int)num_classes, micro};
-#define MB200_GO(T)                                                                                                      \
-    return target_dtype == MB200_I64                                                                                    \
-               ? launch_fused<T, true>(preds, target, target_dtype, (int)n, (int)num_classes, sink, probs_out, logits_flag, err_flag, st) \
-               : launch_fused<T, false>(preds, target, target_dtype, (int)n, (int)num_classes, sink, probs_out, logits_flag, err_flag, st)
-    switch (preds_dtype) {
-        case MB200_F32: MB200_GO(float);
-        case MB200_F16: MB200_GO(__half);
-        case MB200_BF16: MB200_GO(__nv_bfloat16);
-        default: set_error("scores must be f32/f16/bf16 (dtype tag %d)", preds_dtype); return MB200_ERR_INVALID;
-    }
-#undef MB200_GO
+    return with_float_type<kNoF64>(preds_dtype, [&](auto t) {
+        using T = typename decltype(t)::type;
+        return target_dtype == MB200_I64
+                   ? launch_fused<T, true>(preds, target, target_dtype, (int)n, (int)num_classes, sink, probs_out, logits_flag, err_flag, st)
+                   : launch_fused<T, false>(preds, target, target_dtype, (int)n, (int)num_classes, sink, probs_out, logits_flag, err_flag, st);
+    });
 }

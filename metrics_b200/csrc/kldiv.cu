@@ -144,25 +144,20 @@ extern "C" int mb200_kl_divergence_rows(const void* p, const void* q, int dtype,
     MB200_REQUIRE(n >= 0 && d >= 0 && d < (1ll << 31), "bad sizes");
     if (n == 0) return 0;
     MB200_REQUIRE(measures_out && (d == 0 || (p && q)), "NULL pointer");
+    MB200_REQUIRE(is_float_tag(dtype), "distributions must be f32/f16/bf16/f64 (dtype tag %d)", dtype);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     long long grid = (n + 7) / 8;
     const long long cap = (long long)sm_count() * 8;
     if (grid > cap) grid = cap;
-#define MB200_KL(T)                                                                                                    \
-    kl_rows_kernel<T><<<(unsigned)grid, 256, 0, st>>>(reinterpret_cast<const T*>(p), reinterpret_cast<const T*>(q), n, \
-                                                      (int)d, log_prob, reinterpret_cast<T*>(measures_out))
-    switch (dtype) {
-        case MB200_F32: MB200_KL(float); break;
-        case MB200_F16: MB200_KL(__half); break;
-        case MB200_BF16: MB200_KL(__nv_bfloat16); break;
-        case MB200_F64:
-            kl_rows_kernel_f64<<<(unsigned)grid, 256, 0, st>>>(reinterpret_cast<const double*>(p),
-                                                               reinterpret_cast<const double*>(q), n, (int)d, log_prob,
-                                                               reinterpret_cast<double*>(measures_out));
-            break;
-        default: set_error("distributions must be f32/f16/bf16/f64 (dtype tag %d)", dtype); return MB200_ERR_INVALID;
-    }
-#undef MB200_KL
+    with_float_type(dtype, [&](auto t) {
+        using T = typename decltype(t)::type;
+        const T *pt = reinterpret_cast<const T*>(p), *qt = reinterpret_cast<const T*>(q);
+        if constexpr (std::is_same_v<T, double>)
+            kl_rows_kernel_f64<<<(unsigned)grid, 256, 0, st>>>(pt, qt, n, (int)d, log_prob, reinterpret_cast<T*>(measures_out));
+        else
+            kl_rows_kernel<T><<<(unsigned)grid, 256, 0, st>>>(pt, qt, n, (int)d, log_prob, reinterpret_cast<T*>(measures_out));
+        return 0;
+    });
     count_launch();
     return check_cuda(cudaGetLastError(), "kl divergence launch");
 }

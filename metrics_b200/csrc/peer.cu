@@ -142,17 +142,14 @@ extern "C" int mb200_peer_pack_keys_put(const void* preds, int preds_dtype, int6
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const dim3 grid((unsigned)((n_local + 31) / 32), (unsigned)((num_classes + 31) / 32));  // y <= 65535: C < 2^21
     MB200_REQUIRE(grid.y <= 65535u, "more than 2,097,120 classes are not supported (got %lld)", (long long)num_classes);
-#define MB200_PUT(T)                                                                                                   \
-    pack_keys_put_kernel<T><<<grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), (int)n_local, (int)num_classes,    \
-                                                 (int)classes_per_rank, (long long)n_total, (long long)col_offset,     \
-                                                 peer_bases, (long long)keys_offset_bytes)
-    switch (preds_dtype) {
-        case MB200_F32: MB200_PUT(float); break;
-        case MB200_F16: MB200_PUT(__half); break;
-        case MB200_BF16: MB200_PUT(__nv_bfloat16); break;
-        default: set_error("scores must be f32/f16/bf16 (dtype tag %d)", preds_dtype); return MB200_ERR_INVALID;
-    }
-#undef MB200_PUT
+    MB200_REQUIRE(is_float_tag<kNoF64>(preds_dtype), "scores must be f32/f16/bf16 (dtype tag %d)", preds_dtype);
+    with_float_type<kNoF64>(preds_dtype, [&](auto t) {
+        using T = typename decltype(t)::type;
+        pack_keys_put_kernel<T><<<grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), (int)n_local, (int)num_classes,
+                                                     (int)classes_per_rank, (long long)n_total, (long long)col_offset, peer_bases,
+                                                     (long long)keys_offset_bytes);
+        return 0;
+    });
     count_launch();
     return check_cuda(cudaGetLastError(), "peer pack+put launch");
 }

@@ -173,57 +173,42 @@ extern "C" int mb200_regression_sums(const void* preds, const void* target, int 
     int gx = (int)(want < 1 ? 1 : (want > cap ? cap : want));
     if ((int64_t)gx * K * d + 8 > mb200_regression_scratch_doubles(n, d, op)) gx = 1;
     if (n > 0) MB200_REQUIRE(preds && target, "NULL pointer");
+    MB200_REQUIRE(is_float_tag(dtype), "regression inputs must be floating point (dtype tag %d)", dtype);
     if (d == 1 && n > 0) {  // flat vectorised path
         constexpr int per_cta = kRegFlatThreads * 8;
         long long fg = (n + per_cta - 1) / per_cta;
         if (fg > 296) fg = 296;  // scratch holds 296 partial rows
         const int g1 = (int)(fg < 1 ? 1 : fg);
-#define MB200_REG_FLAT(T, DBL, TW)                                                                                          \
-    if (!TW && op == REG_MSE)                                                                                              \
-        reg_flat_kernel<T, DBL, false, REG_MSE><<<g1, kRegFlatThreads, 0, st>>>((const T*)preds, (const T*)target, n, op, param, epsilon, scratch); \
-    else if (!TW && op == REG_MAE)                                                                                         \
-        reg_flat_kernel<T, DBL, false, REG_MAE><<<g1, kRegFlatThreads, 0, st>>>((const T*)preds, (const T*)target, n, op, param, epsilon, scratch); \
-    else                                                                                                                   \
-        reg_flat_kernel<T, DBL, TW><<<g1, kRegFlatThreads, 0, st>>>((const T*)preds, (const T*)target, n, op, param, epsilon, scratch)
-#define MB200_REG_FLAT_BY_DTYPE(TW)                                                                                   \
-    switch (dtype) {                                                                                                  \
-        case MB200_F32: MB200_REG_FLAT(float, false, TW); break;                                                      \
-        case MB200_F64: MB200_REG_FLAT(double, true, TW); break;                                                      \
-        case MB200_F16: MB200_REG_FLAT(__half, false, TW); break;                                                     \
-        case MB200_BF16: MB200_REG_FLAT(__nv_bfloat16, false, TW); break;                                             \
-        default: set_error("regression inputs must be floating point (dtype tag %d)", dtype); return MB200_ERR_INVALID; \
-    }
-        if (op == REG_TWEEDIE) {
-            MB200_REG_FLAT_BY_DTYPE(true)
-        } else {
-            MB200_REG_FLAT_BY_DTYPE(false)
-        }
-#undef MB200_REG_FLAT_BY_DTYPE
-#undef MB200_REG_FLAT
+        with_float_type(dtype, [&](auto t) {
+            using T = typename decltype(t)::type;
+            constexpr bool DBL = std::is_same_v<T, double>;
+            const T *p = (const T*)preds, *q = (const T*)target;
+            if (op == REG_TWEEDIE)
+                reg_flat_kernel<T, DBL, true><<<g1, kRegFlatThreads, 0, st>>>(p, q, n, op, param, epsilon, scratch);
+            else if (op == REG_MSE)
+                reg_flat_kernel<T, DBL, false, REG_MSE><<<g1, kRegFlatThreads, 0, st>>>(p, q, n, op, param, epsilon, scratch);
+            else if (op == REG_MAE)
+                reg_flat_kernel<T, DBL, false, REG_MAE><<<g1, kRegFlatThreads, 0, st>>>(p, q, n, op, param, epsilon, scratch);
+            else
+                reg_flat_kernel<T, DBL, false><<<g1, kRegFlatThreads, 0, st>>>(p, q, n, op, param, epsilon, scratch);
+            return 0;
+        });
         reg_final_kernel<<<1, 256, 0, st>>>(scratch, g1, K, 1, out_sums);
         count_launch();
         count_launch();
         return check_cuda(cudaGetLastError(), "regression sums launch");
     }
     const dim3 grid((unsigned)gx, (unsigned)col_tiles);
-#define MB200_REG_PART(T, DBL, TW)                                                                                      \
-    reg_partial_kernel<T, DBL, TW><<<grid, 256, 0, st>>>((const T*)preds, (const T*)target, n, (int)d, op, param, epsilon, \
-                                                         cols_per_block, scratch)
-#define MB200_REG_PART_BY_DTYPE(TW)                                                                                   \
-    switch (dtype) {                                                                                                  \
-        case MB200_F32: MB200_REG_PART(float, false, TW); break;                                                      \
-        case MB200_F64: MB200_REG_PART(double, true, TW); break;                                                      \
-        case MB200_F16: MB200_REG_PART(__half, false, TW); break;                                                     \
-        case MB200_BF16: MB200_REG_PART(__nv_bfloat16, false, TW); break;                                             \
-        default: set_error("regression inputs must be floating point (dtype tag %d)", dtype); return MB200_ERR_INVALID; \
-    }
-    if (op == REG_TWEEDIE) {
-        MB200_REG_PART_BY_DTYPE(true)
-    } else {
-        MB200_REG_PART_BY_DTYPE(false)
-    }
-#undef MB200_REG_PART_BY_DTYPE
-#undef MB200_REG_PART
+    with_float_type(dtype, [&](auto t) {
+        using T = typename decltype(t)::type;
+        constexpr bool DBL = std::is_same_v<T, double>;
+        const T *p = (const T*)preds, *q = (const T*)target;
+        if (op == REG_TWEEDIE)
+            reg_partial_kernel<T, DBL, true><<<grid, 256, 0, st>>>(p, q, n, (int)d, op, param, epsilon, cols_per_block, scratch);
+        else
+            reg_partial_kernel<T, DBL, false><<<grid, 256, 0, st>>>(p, q, n, (int)d, op, param, epsilon, cols_per_block, scratch);
+        return 0;
+    });
     reg_final_kernel<<<(int)((K * d + 255) / 256), 256, 0, st>>>(scratch, gx, K, (int)d, out_sums);
     count_launch();
     count_launch();

@@ -456,8 +456,6 @@ int launch_onehot_op(int op, const void* preds, const void* target, long long N,
     return launch_onehot<T, MB200_SEG_MUL>(preds, target, N, C, S, layout, p_sn, t_sn, off, Cp, counts, nullptr, 0, st);
 }
 
-bool is_float_tag(int d) { return d == MB200_F32 || d == MB200_F16 || d == MB200_BF16; }
-
 }  // namespace
 }  // namespace mb200
 
@@ -475,13 +473,13 @@ extern "C" int mb200_segmentation_overlap_counts(const void* preds, int preds_dt
     MB200_REQUIRE(num_classes < (1ll << 31), "num_classes exceeds int32");
     MB200_REQUIRE(input_format == MB200_SEG_INDEX || input_format == MB200_SEG_ONE_HOT, "unknown input_format %d", input_format);
     MB200_REQUIRE(op == MB200_SEG_AND || op == MB200_SEG_MUL, "unknown op %d", op);
-    const bool is_float = is_float_tag(preds_dtype);
+    const bool is_float = is_float_tag<kNoF64>(preds_dtype);
     if (input_format == MB200_SEG_INDEX) {
         MB200_REQUIRE(preds_dtype == MB200_I64 && target_dtype == MB200_I64, "index labels must be int64 (dtype tags %d, %d)",
                       preds_dtype, target_dtype);
     } else {
         MB200_REQUIRE(preds_dtype == target_dtype, "preds and target must share a dtype (tags %d, %d)", preds_dtype, target_dtype);
-        MB200_REQUIRE(is_float || (preds_dtype >= MB200_I64 && preds_dtype <= MB200_BOOL), "unsupported dtype tag %d", preds_dtype);
+        MB200_REQUIRE(is_float || is_label_tag(preds_dtype), "unsupported dtype tag %d", preds_dtype);
         MB200_REQUIRE(!is_float || op == MB200_SEG_MUL, "floating-point inputs support only the product");
         MB200_REQUIRE(layout == MB200_SEG_PLANAR || layout == MB200_SEG_CHANNELS_LAST, "unknown layout %d", layout);
     }
@@ -505,16 +503,18 @@ extern "C" int mb200_segmentation_overlap_counts(const void* preds, int preds_dt
         case MB200_I16: return launch_onehot_op<short>(op, preds, target, n, C, inner, layout, p_sn, t_sn, off, Cp, counts, st);
         case MB200_I32: return launch_onehot_op<int>(op, preds, target, n, C, inner, layout, p_sn, t_sn, off, Cp, counts, st);
         case MB200_I64: return launch_onehot_op<long long>(op, preds, target, n, C, inner, layout, p_sn, t_sn, off, Cp, counts, st);
-        case MB200_F32: return launch_onehot<float, MB200_SEG_MUL>(preds, target, n, C, inner, layout, p_sn, t_sn, off, Cp, counts, scratch, scratch_bytes, st);
-        case MB200_F16: return launch_onehot<__half, MB200_SEG_MUL>(preds, target, n, C, inner, layout, p_sn, t_sn, off, Cp, counts, scratch, scratch_bytes, st);
-        default: return launch_onehot<__nv_bfloat16, MB200_SEG_MUL>(preds, target, n, C, inner, layout, p_sn, t_sn, off, Cp, counts, scratch, scratch_bytes, st);
+        default:  // f32 / f16 / bf16: the tag was checked above
+            return with_float_type<kNoF64>(preds_dtype, [&](auto t) {
+                return launch_onehot<typename decltype(t)::type, MB200_SEG_MUL>(preds, target, n, C, inner, layout, p_sn, t_sn, off,
+                                                                                Cp, counts, scratch, scratch_bytes, st);
+            });
     }
 }
 
 extern "C" int64_t mb200_segmentation_scratch_bytes(int64_t n, int64_t num_classes, int64_t inner, int input_format, int layout,
                                                    int dtype, int drop_background) {
     if (n < 0 || inner < 0 || num_classes < 1 || num_classes >= (1ll << 31)) return -1;
-    if (input_format != MB200_SEG_ONE_HOT || !is_float_tag(dtype)) return 0;
+    if (input_format != MB200_SEG_ONE_HOT || !is_float_tag<kNoF64>(dtype)) return 0;
     const int Cp = (int)num_classes - ((drop_background && num_classes > 1) ? 1 : 0);
     return onehot_scratch_bytes(n, Cp, inner, layout, true);
 }
