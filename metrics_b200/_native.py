@@ -141,11 +141,23 @@ SEGMENTATION_SIGNATURES = {
     "mb200_segmentation_scratch_bytes": ("q", "qqqiiii"),
     "mb200_segmentation_overlap_counts": ("i", "pipiqqqiiqqiippqpp"),
 }
+# The retrieval entry points (K16) are declared in include/metrics_b200_retrieval.h, exported from the same library;
+# tests/test_retrieval_abi.py holds this table to that header.
+RETRIEVAL_SIGNATURES = {
+    "mb200_retrieval_index_range": ("i", "pqpp"),
+    "mb200_retrieval_sort_scratch_bytes": ("q", "qi"),
+    "mb200_retrieval_sort": ("i", "pppiqqqpppppqp"),
+    "mb200_retrieval_ideal_scratch_bytes": ("q", "qi"),
+    "mb200_retrieval_sort_ideal": ("i", "ppqippqpp"),
+    "mb200_retrieval_evaluate_scratch_bytes": ("q", "q"),
+    "mb200_retrieval_evaluate": ("i", "pppppqiqipppqp"),
+}
 
 
 def declare_signatures(handle) -> None:
     """Set ``restype`` / ``argtypes`` of every exported function on a loaded library handle."""
-    for name, (ret, args) in (*SIGNATURES.items(), *CALIBRATION_SIGNATURES.items(), *SEGMENTATION_SIGNATURES.items()):
+    for name, (ret, args) in (*SIGNATURES.items(), *CALIBRATION_SIGNATURES.items(), *SEGMENTATION_SIGNATURES.items(),
+                                *RETRIEVAL_SIGNATURES.items()):
         fn = getattr(handle, name)
         fn.restype = _C_TYPES[ret]
         fn.argtypes = [_C_TYPES[a] for a in args]
@@ -1037,3 +1049,107 @@ def segmentation_overlap_counts(preds: Tensor, target: Tensor, num_classes: int,
     if rc:
         check(rc, "segmentation_overlap_counts")
     return counts
+
+
+# ----------------------------------------------------------------------------------------------------------
+# K16 wrappers (retrieval, include/metrics_b200_retrieval.h)
+# ----------------------------------------------------------------------------------------------------------
+RET_AP, RET_RR, RET_PRECISION, RET_RECALL, RET_HIT_RATE, RET_FALL_OUT, RET_R_PRECISION, RET_NDCG = range(8)
+RET_MAX_ELEMENTS = (1 << 30) - 1
+
+
+def _nbytes(v: int) -> int:
+    return (int(v).bit_length() + 7) // 8
+
+
+class RetrievalGroups:
+    """Records sorted by (index, score descending, position) and the query boundaries: the output of one group sort."""
+
+    def __init__(self, keys: Tensor, target: Tensor, offsets: Tensor, info: Tensor, num_queries: int, segment_bytes: int):
+        self.keys, self.target, self.offsets, self.info = keys, target, offsets, info
+        self.num_queries, self.segment_bytes = num_queries, segment_bytes
+
+
+def retrieval_sort_scratch_bytes(n: int, index_bytes: int) -> int:
+    """Workspace of the group sort; raises ValueError above 2^30 - 1 records (the radix sort counts in 30 bits)."""
+    nbytes = int(lib().mb200_retrieval_sort_scratch_bytes(int(n), int(index_bytes)))
+    if nbytes < 0:
+        raise ValueError(f"metrics_b200: retrieval metrics support at most 2^30 - 1 = {RET_MAX_ELEMENTS} elements in total, "
+                         f"got {n}.")
+    return nbytes
+
+
+def retrieval_sort(indexes: Optional[Tensor], preds: Tensor, target: Tensor) -> RetrievalGroups:
+    """K16a + K16b: group ``preds`` / ``target`` by ``indexes`` (``None``: one query) in ascending index order, each query by
+    descending score, ties in input order.  Reads the index range and the query count back (two host synchronisations;
+    one when ``indexes`` is None)."""
+    dev = require_cuda(preds, target) if indexes is None else require_cuda(indexes, preds, target)
+    n = preds.numel()
+    preds = preds.reshape(-1).to(torch.float32).contiguous()
+    target = target.reshape(-1)
+    target = (target.to(torch.float32) if target.is_floating_point() else target.to(torch.int64)).contiguous()
+    lib_ = lib()
+    retrieval_sort_scratch_bytes(n, 0)  # the size guard, before anything is allocated
+    st = stream_handle(dev)
+    if indexes is None:
+        indexes = torch.zeros(n, dtype=torch.int64, device=dev)
+        lo, hi = 0, 0
+    else:
+        indexes = indexes.reshape(-1).to(torch.int64).contiguous()
+        rng = torch.empty(2, dtype=torch.int64, device=dev)
+        with on_device(dev):
+            check(lib_.mb200_retrieval_index_range(indexes.data_ptr(), n, rng.data_ptr(), st), "retrieval_index_range")
+        lo, hi = rng.tolist()
+    index_bytes = _nbytes(hi - lo)
+    nbytes = retrieval_sort_scratch_bytes(n, index_bytes)
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    keys = torch.empty(n, dtype=torch.int64, device=dev)
+    sorted_target = torch.empty(n, dtype=torch.float32, device=dev)
+    offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    info = torch.zeros(2, dtype=torch.int64, device=dev)
+    with on_device(dev):
+        rc = lib_.mb200_retrieval_sort(indexes.data_ptr(), preds.data_ptr(), target.data_ptr(), tag(target), n, lo, hi,
+                                       keys.data_ptr(), sorted_target.data_ptr(), offsets.data_ptr(), info.data_ptr(),
+                                       scratch.data_ptr(), nbytes, st)
+    check(rc, "retrieval_sort")
+    q, flags = info.tolist()
+    if flags & FLAG_SPIN_TIMEOUT:
+        raise NativeLibraryError("metrics_b200.retrieval_sort: the radix sort's look-back wait expired (results invalid)")
+    segment_bytes = index_bytes if index_bytes <= 4 else _nbytes(q - 1)
+    return RetrievalGroups(keys, sorted_target, offsets, info, int(q), segment_bytes)
+
+
+def retrieval_sort_ideal(groups: RetrievalGroups) -> Tensor:
+    """K16c: every query's targets in descending order (the ideal ranking of NDCG), float32 ``[n]``."""
+    dev = groups.keys.device
+    n = groups.keys.numel()
+    lib_ = lib()
+    nbytes = int(lib_.mb200_retrieval_ideal_scratch_bytes(n, groups.segment_bytes))
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    ideal = torch.empty(n, dtype=torch.float32, device=dev)
+    err = torch.zeros(1, dtype=torch.int32, device=dev)
+    with on_device(dev):
+        rc = lib_.mb200_retrieval_sort_ideal(groups.keys.data_ptr(), groups.target.data_ptr(), n, groups.segment_bytes,
+                                             ideal.data_ptr(), scratch.data_ptr(), nbytes, err.data_ptr(), stream_handle(dev))
+    check(rc, "retrieval_sort_ideal")
+    return ideal
+
+
+def retrieval_evaluate(groups: RetrievalGroups, kind: int, top_k: Optional[int] = None, adaptive_k: bool = False,
+                       ideal: Optional[Tensor] = None) -> tuple[Tensor, Tensor]:
+    """K16d: ``(value float32 [Q], empty bool [Q])`` of metric ``kind`` per query, in ascending index order.  ``top_k``
+    None (or 0) means the query length.  No host synchronisation."""
+    dev = groups.keys.device
+    n = groups.keys.numel()
+    q = groups.num_queries
+    lib_ = lib()
+    nbytes = int(lib_.mb200_retrieval_evaluate_scratch_bytes(n))
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    value = torch.empty(max(q, 1), dtype=torch.float32, device=dev)
+    empty = torch.empty(max(q, 1), dtype=torch.uint8, device=dev)
+    with on_device(dev):
+        rc = lib_.mb200_retrieval_evaluate(groups.keys.data_ptr(), groups.target.data_ptr(), ptr(ideal), groups.offsets.data_ptr(),
+                                           groups.info.data_ptr(), n, int(kind), int(top_k or 0), int(bool(adaptive_k)),
+                                           value.data_ptr(), empty.data_ptr(), scratch.data_ptr(), nbytes, stream_handle(dev))
+    check(rc, "retrieval_evaluate")
+    return value[:q], empty[:q].bool()

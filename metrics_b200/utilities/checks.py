@@ -95,3 +95,48 @@ def check_forward_full_state_property(metric_class, init_args=None, input_args=N
         print(f"Full state for {steps} steps took: {mean[0, j]}+-{std[0, j]:0.3f}")
         print(f"Partial state for {steps} steps took: {mean[1, j]:0.3f}+-{std[1, j]:0.3f}")
     print(f"Recommended setting `full_state_update={not bool(mean[1, -1] < mean[0, -1])}`")
+
+
+def _check_retrieval_functional_inputs(preds: Tensor, target: Tensor, allow_non_binary_target: bool = False):
+    """``(preds float32, target int64 or float32)``, flattened, of one query (reference checks.py:508-536): same shape,
+    non-empty, then `_check_retrieval_target_and_prediction_types`."""
+    if preds.shape != target.shape:
+        raise ValueError("`preds` and `target` must be of the same shape")
+    if not preds.numel() or not preds.size():
+        raise ValueError("`preds` and `target` must be non-empty and non-scalar tensors")
+    return _check_retrieval_target_and_prediction_types(preds, target, allow_non_binary_target=allow_non_binary_target)
+
+
+def _check_retrieval_inputs(indexes: Tensor, preds: Tensor, target: Tensor, allow_non_binary_target: bool = False,
+                            ignore_index=None):
+    """``(indexes int64, preds float32, target)`` flattened, with the records whose target is ``ignore_index`` removed
+    (reference checks.py:539-585).  The ``ignore_index`` mask and the binary-target check read values on the host."""
+    import torch
+
+    if indexes.shape != preds.shape or preds.shape != target.shape:
+        raise ValueError("`indexes`, `preds` and `target` must be of the same shape")
+    if indexes.dtype is not torch.long:
+        raise ValueError("`indexes` must be a tensor of long integers")
+    if ignore_index is not None:
+        keep = target != ignore_index
+        indexes, preds, target = indexes[keep], preds[keep], target[keep]
+    if not indexes.numel() or not indexes.size():
+        raise ValueError("`indexes`, `preds` and `target` must be non-empty and non-scalar tensors")
+    preds, target = _check_retrieval_target_and_prediction_types(preds, target, allow_non_binary_target=allow_non_binary_target)
+    return indexes.long().flatten(), preds, target
+
+
+def _check_retrieval_target_and_prediction_types(preds: Tensor, target: Tensor, allow_non_binary_target: bool = False):
+    """Dtype checks of a retrieval batch (reference checks.py:588-615): bool / int32 / int64 / floating targets, floating
+    scores, binary targets unless ``allow_non_binary_target``.  Returns flat ``preds`` float32 and ``target`` float32 when
+    floating, else int64."""
+    import torch
+
+    if target.dtype not in (torch.bool, torch.long, torch.int) and not torch.is_floating_point(target):
+        raise ValueError("`target` must be a tensor of booleans, integers or floats")
+    if not preds.is_floating_point():
+        raise ValueError("`preds` must be a tensor of floats")
+    if not allow_non_binary_target and (target.max() > 1 or target.min() < 0):
+        raise ValueError("`target` must contain `binary` values")
+    target = target.float() if target.is_floating_point() else target.long()
+    return preds.float().flatten(), target.flatten()
