@@ -7,6 +7,7 @@
  *   retrieval/base.py:148-183        sort by indexes, _flexible_bincount(...).cpu(), Python loop over the queries
  *   retrieval/fall_out.py:117-155    the same loop with "no negative target" emptiness
  *   functional/retrieval/*.py        the per-query topk / argsort / gather / sum of each metric
+ *   retrieval/precision_recall_curve.py:205-256   the per-query curve loop and its [Q, max_k] stack
  */
 #ifndef METRICS_B200_RETRIEVAL_H_
 #define METRICS_B200_RETRIEVAL_H_
@@ -73,6 +74,30 @@ MB200_API int mb200_retrieval_evaluate(const uint64_t* keys, const float* sorted
                                        const int64_t* offsets, const int64_t* num_queries, int64_t n, int kind, int64_t top_k,
                                        int adaptive_k, float* value, uint8_t* empty, void* scratch, int64_t scratch_bytes,
                                        void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * K16e — AUROC of each query's top min(top_k, n) records (top_k = 0: all), over the output of K16b.  value[q] float32:
+ * 0 when the slice has no target equal to 0 or none equal to 1; else binary_auroc of the slice with positives = targets
+ * equal to 1, every score replaced by its fp32 sigmoid when a non-NaN score of the slice lies outside [0, 1], ties averaged,
+ * each NaN its own group.  max_fpr < 0 or == 1: the full area; else the McClish-standardised partial area up to max_fpr
+ * (which must round to a float32 below 1; 0 gives NaN).  empty[q] = 1 when the whole query has no positive target.
+ * scratch: mb200_retrieval_evaluate_scratch_bytes(n) bytes.  Same scheduling and determinism as K16d.
+ * ------------------------------------------------------------------------------------------------ */
+MB200_API int mb200_retrieval_auroc(const uint64_t* keys, const float* sorted_target, const int64_t* offsets,
+                                    const int64_t* num_queries, int64_t n, int64_t top_k, double max_fpr, float* value,
+                                    uint8_t* empty, void* scratch, int64_t scratch_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * K16f — precision and recall at k = 1..max_k (max_k >= 1) of each query, over the output of K16b.  precision and recall
+ * are row-major [num_queries, max_k] float32 (int64 indexing).  With cum(k) = the target sum of the top min(k, n)
+ * records and P = the query's target sum: precision[q, k-1] = cum(k) / d, d = k (adaptive_k and k > n: n), recall[q, k-1]
+ * = cum(k) / P, fp32 divisions.  empty[q] = 1 when P == 0; its row is zeros.  scratch:
+ * mb200_retrieval_pr_curve_scratch_bytes(n) bytes.
+ * ------------------------------------------------------------------------------------------------ */
+MB200_API int64_t mb200_retrieval_pr_curve_scratch_bytes(int64_t n);
+MB200_API int mb200_retrieval_pr_curve(const uint64_t* keys, const float* sorted_target, const int64_t* offsets,
+                                       const int64_t* num_queries, int64_t n, int64_t max_k, int adaptive_k, float* precision,
+                                       float* recall, uint8_t* empty, void* scratch, int64_t scratch_bytes, void* stream);
 
 #ifdef __cplusplus
 }

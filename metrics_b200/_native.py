@@ -151,6 +151,9 @@ RETRIEVAL_SIGNATURES = {
     "mb200_retrieval_sort_ideal": ("i", "ppqippqpp"),
     "mb200_retrieval_evaluate_scratch_bytes": ("q", "q"),
     "mb200_retrieval_evaluate": ("i", "pppppqiqipppqp"),
+    "mb200_retrieval_auroc": ("i", "ppppqqdpppqp"),
+    "mb200_retrieval_pr_curve_scratch_bytes": ("q", "q"),
+    "mb200_retrieval_pr_curve": ("i", "ppppqqippppqp"),
 }
 
 
@@ -1153,3 +1156,42 @@ def retrieval_evaluate(groups: RetrievalGroups, kind: int, top_k: Optional[int] 
                                            value.data_ptr(), empty.data_ptr(), scratch.data_ptr(), nbytes, stream_handle(dev))
     check(rc, "retrieval_evaluate")
     return value[:q], empty[:q].bool()
+
+
+def retrieval_auroc(groups: RetrievalGroups, top_k: Optional[int] = None, max_fpr: Optional[float] = None) -> tuple[Tensor, Tensor]:
+    """K16e: ``(value float32 [Q], empty bool [Q])``: the AUROC of each query's top ``top_k`` records (None: all), the
+    partial, McClish-standardised area up to ``max_fpr`` unless it is None or 1.  No host synchronisation."""
+    dev = groups.keys.device
+    n = groups.keys.numel()
+    q = groups.num_queries
+    lib_ = lib()
+    nbytes = int(lib_.mb200_retrieval_evaluate_scratch_bytes(n))
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    value = torch.empty(max(q, 1), dtype=torch.float32, device=dev)
+    empty = torch.empty(max(q, 1), dtype=torch.uint8, device=dev)
+    with on_device(dev):
+        rc = lib_.mb200_retrieval_auroc(groups.keys.data_ptr(), groups.target.data_ptr(), groups.offsets.data_ptr(),
+                                        groups.info.data_ptr(), n, int(top_k or 0), -1.0 if max_fpr is None else float(max_fpr),
+                                        value.data_ptr(), empty.data_ptr(), scratch.data_ptr(), nbytes, stream_handle(dev))
+    check(rc, "retrieval_auroc")
+    return value[:q], empty[:q].bool()
+
+
+def retrieval_pr_curve(groups: RetrievalGroups, max_k: int, adaptive_k: bool = False) -> tuple[Tensor, Tensor, Tensor]:
+    """K16f: ``(precision float32 [Q, max_k], recall float32 [Q, max_k], empty bool [Q])`` at k = 1..max_k per query; the
+    rows of queries without a positive target are zeros.  No host synchronisation."""
+    dev = groups.keys.device
+    n = groups.keys.numel()
+    q = groups.num_queries
+    lib_ = lib()
+    nbytes = int(lib_.mb200_retrieval_pr_curve_scratch_bytes(n))
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    precision = torch.empty((max(q, 1), max_k), dtype=torch.float32, device=dev)
+    recall = torch.empty((max(q, 1), max_k), dtype=torch.float32, device=dev)
+    empty = torch.empty(max(q, 1), dtype=torch.uint8, device=dev)
+    with on_device(dev):
+        rc = lib_.mb200_retrieval_pr_curve(groups.keys.data_ptr(), groups.target.data_ptr(), groups.offsets.data_ptr(),
+                                           groups.info.data_ptr(), n, int(max_k), int(bool(adaptive_k)), precision.data_ptr(),
+                                           recall.data_ptr(), empty.data_ptr(), scratch.data_ptr(), nbytes, stream_handle(dev))
+    check(rc, "retrieval_pr_curve")
+    return precision[:q], recall[:q], empty[:q].bool()

@@ -111,6 +111,10 @@ __device__ __forceinline__ float f32_from_order_key(unsigned k) {
     return __uint_as_float(b);
 }
 
+// The logistic function in fp32 math, as ATen's CUDA sigmoid computes it (the logits-to-probabilities step of
+// normalize_logits_if_needed); NaN stays NaN.
+__device__ __forceinline__ float sigmoid_f32(float v) { return 1.0f / (1.0f + expf(-v)); }
+
 __device__ __forceinline__ unsigned long long f64_order_key(double v) {
     unsigned long long b = (unsigned long long)__double_as_longlong(v);
     if ((b & 0x7fffffffffffffffull) > 0x7ff0000000000000ull) return ~0ull;

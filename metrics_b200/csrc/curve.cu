@@ -123,7 +123,7 @@ __global__ void __launch_bounds__(256) sigmoid_if_kernel(const T* __restrict__ x
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
         if (apply) {
             const float v = to_float<T>(x[i]);
-            out[i] = from_float<T>(1.0f / (1.0f + expf(-v)));  // fp32 math, rounded to T like ATen's sigmoid
+            out[i] = from_float<T>(sigmoid_f32(v));  // fp32 math, rounded to T like ATen's sigmoid
         } else {
             out[i] = x[i];
         }
@@ -195,14 +195,14 @@ __global__ void __launch_bounds__(256) sigmoid_spec_kernel(const T* __restrict__
                 if (apply) {
                     T* e = reinterpret_cast<T*>(&q[k]);
 #pragma unroll
-                    for (int j = 0; j < kVec; ++j) e[j] = from_float<T>(1.0f / (1.0f + expf(-to_float<T>(e[j]))));
+                    for (int j = 0; j < kVec; ++j) e[j] = from_float<T>(sigmoid_f32(to_float<T>(e[j])));
                 }
                 ov[v] = q[k];
             }
         }
         if (last)
             for (long long i = nvec * kVec + threadIdx.x; i < n; i += 256)
-                out[i] = apply ? from_float<T>(1.0f / (1.0f + expf(-to_float<T>(x[i])))) : x[i];
+                out[i] = apply ? from_float<T>(sigmoid_f32(to_float<T>(x[i]))) : x[i];
     }
 }
 
@@ -240,7 +240,7 @@ __global__ void __launch_bounds__(1024) sigmoid_if_small_kernel(const T* __restr
             } else if constexpr (sizeof(T) == 8) {
                 out[i] = (T)(1.0 / (1.0 + exp(-(double)v[k])));
             } else {
-                out[i] = from_float<T>(1.0f / (1.0f + expf(-to_float<T>(v[k]))));
+                out[i] = from_float<T>(sigmoid_f32(to_float<T>(v[k])));
             }
         }
     }

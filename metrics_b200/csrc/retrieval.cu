@@ -1,4 +1,5 @@
-// K16 — retrieval metrics (MAP, MRR, Precision, Recall, HitRate, FallOut, R-Precision, NDCG) on sm_90a.
+// K16 — retrieval metrics (MAP, MRR, Precision, Recall, HitRate, FallOut, R-Precision, NDCG, AUROC, precision-recall curve)
+// on sm_90a.
 //
 // Reference replaced (src/torchmetrics/): retrieval/base.py:148-183 sorts by `indexes`, moves the group sizes to the host
 // and runs a Python loop over the queries, each with its own topk / argsort, gathers and sums (functional/retrieval/*.py).
@@ -14,7 +15,8 @@
 // listed by the warp kernel and taken in a persistent loop.  Every group walks its query in chunks of one record per
 // thread, with warp-shuffle scans, carries in registers and sums in float64 in a fixed order: deterministic.  NDCG's tie
 // groups (equal score keys) may span chunks: a max-scan of head positions finds the run start, and the run's target sum and
-// discount sum come from prefix differences.
+// discount sum come from prefix differences.  AUROC (K16e) and the precision-recall curve (K16f) are further per-query
+// bodies on the same scheduling; the curve's columns past each query's length are filled by a separate flat kernel.
 #include <algorithm>
 
 #include "common.cuh"
@@ -394,7 +396,18 @@ __device__ void eval_query(const EvalArgs& a, long long q, const Group<G>& g) {
     }
 }
 
-__global__ void __launch_bounds__(kThreads) eval_warp_kernel(EvalArgs a, const long long* __restrict__ num_queries,
+// The per-query bodies: `body(q, g)` evaluates query q with the G threads of g; `body.offsets` are the query offsets.
+struct MetricBody {
+    EvalArgs a;
+    const long long* offsets;
+    template <int G>
+    __device__ __forceinline__ void operator()(long long q, const Group<G>& g) const {
+        eval_query<G>(a, q, g);
+    }
+};
+
+template <class Body>
+__global__ void __launch_bounds__(kThreads) eval_warp_kernel(Body body, const long long* __restrict__ num_queries,
                                                              unsigned* __restrict__ long_list, unsigned* __restrict__ long_count) {
     __shared__ GroupSmem<32> sm[kThreads / 32];
     const int warp = threadIdx.x >> 5;
@@ -402,23 +415,210 @@ __global__ void __launch_bounds__(kThreads) eval_warp_kernel(EvalArgs a, const l
     const long long nq = *num_queries;
     const long long stride = (long long)gridDim.x * (kThreads / 32);
     for (long long q = (long long)blockIdx.x * (kThreads / 32) + warp; q < nq; q += stride) {
-        if (a.offsets[q + 1] - a.offsets[q] > kLongQuery) {
+        if (body.offsets[q + 1] - body.offsets[q] > kLongQuery) {
             if (g.r == 0) long_list[atomicAdd(long_count, 1u)] = (unsigned)q;
             continue;
         }
-        eval_query<32>(a, q, g);
+        body(q, g);
     }
 }
 
-__global__ void __launch_bounds__(kCtaThreads) eval_cta_kernel(EvalArgs a, const unsigned* __restrict__ long_list,
+template <class Body>
+__global__ void __launch_bounds__(kCtaThreads) eval_cta_kernel(Body body, const unsigned* __restrict__ long_list,
                                                                const unsigned* __restrict__ long_count) {
     __shared__ GroupSmem<kCtaThreads> sm;
     Group<kCtaThreads> g{(int)threadIdx.x, &sm};
     const unsigned count = *long_count;
-    for (unsigned j = blockIdx.x; j < count; j += gridDim.x) eval_query<kCtaThreads>(a, long_list[j], g);
+    for (unsigned j = blockIdx.x; j < count; j += gridDim.x) body((long long)long_list[j], g);
+}
+
+// ---- K16e: AUROC of each query's top min(top_k, n) records ---------------------------------------------------------------
+// restates retrieval_auroc -> binary_auroc: a slice without a target equal to 0 or without one equal to 1 scores 0; a
+// positive is a target equal to 1; when any (non-NaN) score of the slice lies outside [0, 1] every score is replaced by its
+// fp32 sigmoid before the tie groups (runs of equal values, each NaN its own group) are formed.  The full area is the exact
+// integer sum_g fp_g * (2 TP_before + tp_g) over 2 P N.  The partial area stops at the first ROC point whose fp32 FPR
+// exceeds max_fpr (rounded to fp32), interpolates TPR linearly there and takes McClish's standardisation.
+struct AurocBody {
+    const u64* keys;
+    const float* tgt;
+    const long long* offsets;
+    long long top_k;
+    double max_fpr;  // < 0: the full area
+    float* value;
+    unsigned char* empty;
+
+    template <int G>
+    __device__ void operator()(long long q, const Group<G>& g) const {
+        const long long s = offsets[q], n = offsets[q + 1] - s;
+        const u64* k = keys + s;
+        const float* t = tgt + s;
+        const long long len = top_k == 0 ? n : min(top_k, n);
+        double tsum = 0.0;
+        long long has0 = 0, has1 = 0, logit = 0;
+        for (long long i = g.r; i < n; i += G) {
+            const float ti = t[i];
+            tsum += (double)ti;
+            if (i < len) {
+                const float v = f32_from_order_key(~(unsigned)k[i]);
+                has0 |= ti == 0.0f;
+                has1 |= ti == 1.0f;
+                logit |= v < 0.0f || v > 1.0f;
+            }
+        }
+        tsum = g.sum(tsum);
+        has0 = g.sum(has0);
+        has1 = g.sum(has1);
+        logit = g.sum(logit);
+        double v = 0.0;
+        if (has0 && has1) {
+            const bool sig = logit != 0;
+            auto score = [k, sig](long long i) {
+                const float x = f32_from_order_key(~(unsigned)k[i]);
+                return sig ? sigmoid_f32(x) : x;
+            };
+            long long npos = 0;
+            for (long long i = g.r; i < len; i += G) npos += t[i] == 1.0f;
+            const long long P = g.sum(npos), N = len - P;
+            const bool partial = max_fpr >= 0.0;
+            const float m32 = (float)max_fpr;
+            const float nf = (float)N;
+            // area: exact sum of fp_g (2 TP_before + tp_g) over the groups that end at or before the crossing point
+            unsigned long long area = 0;
+            long long cfp0 = 0, cfp1 = 0, ctp0 = 0, ctp1 = 0;  // the crossing segment, held by the one rank that ends it
+            long long carry = 0, head_tp = 0, head_pos = 0;
+            double* sx = g.sm->s;
+            for (long long base = 0; base < len; base += G) {
+                const long long i = base + g.r;
+                const bool valid = i < len;
+                const float w = valid ? score(i) : 0.0f;
+                const long long pos = valid && t[i] == 1.0f;
+                const bool head = valid && (i == 0 || !(score(i - 1) == w));
+                const bool end = valid && (i == len - 1 || !(score(i + 1) == w));
+                const long long tp = carry + g.scan(pos, [](long long x, long long y) { return x + y; });
+                sx[g.r] = (double)(tp - pos);  // exclusive TP count at this rank
+                const int hp = g.smax(head ? g.r : -1);
+                g.bar();
+                if (end) {
+                    long long tp0 = head_tp, a0 = head_pos;
+                    if (hp >= 0) {
+                        tp0 = (long long)sx[hp];
+                        a0 = base + hp;
+                    }
+                    const long long fp0 = a0 - tp0, fp1 = i + 1 - tp;
+                    const unsigned long long contrib = (unsigned long long)(fp1 - fp0) * (unsigned long long)(tp0 + tp);
+                    if (!partial || (float)fp1 / nf <= m32) {
+                        area += contrib;
+                    } else if ((float)fp0 / nf <= m32) {  // the first ROC point past max_fpr
+                        cfp0 = fp0, cfp1 = fp1, ctp0 = tp0, ctp1 = tp;
+                    }
+                }
+                const int hl = g.last(hp);
+                if (hl >= 0) {
+                    head_tp = (long long)sx[hl];
+                    head_pos = base + hl;
+                }
+                carry = g.last(tp);
+                g.bar();
+            }
+            area = g.sum(area);
+            const double full = (double)area / (2.0 * (double)P * (double)N);
+            if (!partial) {
+                v = full;
+            } else {
+                const double x0 = (double)g.sum(cfp0) / (double)N, x1 = (double)g.sum(cfp1) / (double)N;
+                const double y0 = (double)g.sum(ctp0) / (double)P, y1 = (double)g.sum(ctp1) / (double)P;
+                const double m = (double)m32, min_area = 0.5 * m * m;
+                const double y = y0 + (m - x0) / (x1 - x0) * (y1 - y0);  // TPR interpolated at max_fpr
+                v = 0.5 * (1.0 + (full + (m - x0) * (y0 + y) * 0.5 - min_area) / (m - min_area));
+            }
+        }
+        if (g.r == 0) {
+            value[q] = (float)v;
+            empty[q] = tsum == 0.0;
+        }
+    }
+};
+
+// ---- K16f: precision / recall at k = 1..max_k of each query ---------------------------------------------------------------
+// The per-query body writes the columns k <= min(n, max_k) (a scan of the query's head) and keeps P; the columns past n,
+// where the cumulative count stays P, are written by pr_tail_kernel over the whole matrix so that short queries with a long
+// max_k spread over every SM.  cum(k) / d and cum(k) / P are fp32 divisions of exact counts, as in the reference.
+struct PrCurveBody {
+    const float* tgt;
+    const long long* offsets;
+    long long max_k;
+    float* precision;
+    float* recall;
+    unsigned char* empty;
+    float* positives;  // [Q] scratch: P as float32, for the tail
+
+    template <int G>
+    __device__ void operator()(long long q, const Group<G>& g) const {
+        const long long s = offsets[q], n = offsets[q + 1] - s;
+        const float* t = tgt + s;
+        double tsum = 0.0;
+        for (long long i = g.r; i < n; i += G) tsum += (double)t[i];
+        tsum = g.sum(tsum);
+        const float pf = (float)tsum;
+        const bool none = tsum == 0.0;
+        float* prow = precision + q * max_k;
+        float* rrow = recall + q * max_k;
+        const long long len = min(n, max_k);
+        double carry = 0.0;
+        for (long long base = 0; base < len; base += G) {
+            const long long i = base + g.r;
+            const double ti = i < len ? (double)t[i] : 0.0;
+            const double cum = carry + g.scan(ti, [](double x, double y) { return x + y; });
+            if (i < len) {
+                const float c = (float)cum;
+                prow[i] = none ? 0.0f : c / (float)(i + 1);
+                rrow[i] = none ? 0.0f : c / pf;
+            }
+            carry = g.last(cum);
+        }
+        if (g.r == 0) {
+            positives[q] = pf;
+            empty[q] = none;
+        }
+    }
+};
+
+// columns c >= n of every row, in blocks of kThreads columns: cum = P, d = k (adaptive_k: n)
+__global__ void __launch_bounds__(kThreads) pr_tail_kernel(const long long* __restrict__ offsets, const long long* __restrict__ num_queries,
+                                                           long long max_k, int adaptive_k, const float* __restrict__ positives,
+                                                           float* __restrict__ precision, float* __restrict__ recall) {
+    const long long col_blocks = (max_k + kThreads - 1) / kThreads;
+    const long long units = *num_queries * col_blocks;
+    for (long long u = blockIdx.x; u < units; u += gridDim.x) {
+        const long long q = u / col_blocks;
+        const long long c = (u - q * col_blocks) * kThreads + threadIdx.x;
+        const long long n = offsets[q + 1] - offsets[q];
+        if (c >= max_k || c < n) continue;
+        const float pf = positives[q];
+        const bool none = pf == 0.0f;
+        const long long d = adaptive_k ? n : c + 1;
+        precision[q * max_k + c] = none ? 0.0f : pf / (float)d;
+        recall[q * max_k + c] = none ? 0.0f : pf / pf;
+    }
 }
 
 int grid_for(long long n) { return (int)std::max(1ll, std::min((n + kThreads - 1) / kThreads, (long long)sm_count() * 16)); }
+
+// Warp per query of up to kLongQuery records, listed CTA per longer one: one memset and two launches on `st`.
+// scratch: the long-query count (16 bytes) then the list, mb200_retrieval_evaluate_scratch_bytes(n) bytes in all.
+template <class Body>
+int launch_per_query(const Body& body, const long long* num_queries, long long n, void* scratch, cudaStream_t st) {
+    unsigned* long_count = reinterpret_cast<unsigned*>(scratch);
+    unsigned* long_list = reinterpret_cast<unsigned*>(reinterpret_cast<unsigned char*>(scratch) + 16);
+    MB200_CUDA_OK(cudaMemsetAsync(long_count, 0, 4, st));
+    const int wgrid = (int)std::max(1ll, std::min((long long)(n + kThreads / 32 - 1) / (kThreads / 32), (long long)sm_count() * 16));
+    eval_warp_kernel<Body><<<wgrid, kThreads, 0, st>>>(body, num_queries, long_list, long_count);
+    count_launch();
+    const int cgrid = (int)std::max(1ll, std::min((long long)n / kLongQuery, (long long)sm_count() * 2));
+    eval_cta_kernel<Body><<<cgrid, kCtaThreads, 0, st>>>(body, long_list, long_count);
+    count_launch();
+    return 0;
+}
 
 size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
 
@@ -589,17 +789,54 @@ extern "C" int mb200_retrieval_evaluate(const uint64_t* keys, const float* sorte
     MB200_REQUIRE(keys && sorted_target && offsets && num_queries && value && empty && scratch, "NULL pointer");
     MB200_REQUIRE(kind != MB200_RET_NDCG || ideal, "NDCG needs the ideal order");
     MB200_REQUIRE(scratch_bytes >= need, "scratch too small (%lld < %lld bytes)", (long long)scratch_bytes, (long long)need);
+    const long long* off = reinterpret_cast<const long long*>(offsets);
+    EvalArgs a{reinterpret_cast<const u64*>(keys), sorted_target, ideal, off, kind, (long long)top_k, adaptive_k, value, empty};
+    const int rc = launch_per_query(MetricBody{a, off}, reinterpret_cast<const long long*>(num_queries), n, scratch,
+                                    reinterpret_cast<cudaStream_t>(stream));
+    return rc ? rc : check_cuda(cudaGetLastError(), "retrieval_evaluate");
+}
+
+extern "C" int mb200_retrieval_auroc(const uint64_t* keys, const float* sorted_target, const int64_t* offsets,
+                                     const int64_t* num_queries, int64_t n, int64_t top_k, double max_fpr, float* value,
+                                     uint8_t* empty, void* scratch, int64_t scratch_bytes, void* stream) {
+    MB200_REQUIRE(top_k >= 0, "top_k must be >= 0 (0: the query length), got %lld", (long long)top_k);
+    MB200_REQUIRE(max_fpr < 0.0 || max_fpr == 1.0 || (float)max_fpr < 1.0f,
+                  "max_fpr must be negative (none), 1, or round to a float32 below 1; got %g", max_fpr);
+    const int64_t need = mb200_retrieval_evaluate_scratch_bytes(n);
+    MB200_REQUIRE(need > 0, "bad size %lld", (long long)n);
+    MB200_REQUIRE(keys && sorted_target && offsets && num_queries && value && empty && scratch, "NULL pointer");
+    MB200_REQUIRE(scratch_bytes >= need, "scratch too small (%lld < %lld bytes)", (long long)scratch_bytes, (long long)need);
+    const long long* off = reinterpret_cast<const long long*>(offsets);
+    const AurocBody body{reinterpret_cast<const u64*>(keys), sorted_target, off, (long long)top_k, max_fpr == 1.0 ? -1.0 : max_fpr,
+                         value, empty};
+    const int rc = launch_per_query(body, reinterpret_cast<const long long*>(num_queries), n, scratch,
+                                    reinterpret_cast<cudaStream_t>(stream));
+    return rc ? rc : check_cuda(cudaGetLastError(), "retrieval_auroc");
+}
+
+extern "C" int64_t mb200_retrieval_pr_curve_scratch_bytes(int64_t n) {
+    const int64_t eval = mb200_retrieval_evaluate_scratch_bytes(n);
+    return eval < 0 ? -1 : eval + (int64_t)align16((size_t)n * 4);
+}
+
+extern "C" int mb200_retrieval_pr_curve(const uint64_t* keys, const float* sorted_target, const int64_t* offsets, const int64_t* num_queries, int64_t n,
+                                        int64_t max_k, int adaptive_k, float* precision, float* recall, uint8_t* empty,
+                                        void* scratch, int64_t scratch_bytes, void* stream) {
+    MB200_REQUIRE(max_k >= 1, "max_k must be >= 1, got %lld", (long long)max_k);
+    const int64_t need = mb200_retrieval_pr_curve_scratch_bytes(n);
+    MB200_REQUIRE(need > 0, "bad size %lld", (long long)n);
+    MB200_REQUIRE(keys && sorted_target && offsets && num_queries && precision && recall && empty && scratch, "NULL pointer");
+    MB200_REQUIRE(scratch_bytes >= need, "scratch too small (%lld < %lld bytes)", (long long)scratch_bytes, (long long)need);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    unsigned* long_count = reinterpret_cast<unsigned*>(scratch);
-    unsigned* long_list = reinterpret_cast<unsigned*>(reinterpret_cast<unsigned char*>(scratch) + 16);
-    EvalArgs a{reinterpret_cast<const u64*>(keys), sorted_target, ideal, reinterpret_cast<const long long*>(offsets), kind,
-               (long long)top_k, adaptive_k, value, empty};
-    MB200_CUDA_OK(cudaMemsetAsync(long_count, 0, 4, st));
-    const int wgrid = (int)std::max(1ll, std::min((long long)(n + kThreads / 32 - 1) / (kThreads / 32), (long long)sm_count() * 16));
-    eval_warp_kernel<<<wgrid, kThreads, 0, st>>>(a, reinterpret_cast<const long long*>(num_queries), long_list, long_count);
+    const long long* off = reinterpret_cast<const long long*>(offsets);
+    const long long* nq = reinterpret_cast<const long long*>(num_queries);
+    float* positives = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(scratch) + mb200_retrieval_evaluate_scratch_bytes(n));
+    const PrCurveBody body{sorted_target, off, (long long)max_k, precision, recall, empty, positives};
+    int rc = launch_per_query(body, nq, n, scratch, st);
+    if (rc) return rc;
+    // the tail: up to Q * max_k values whatever the query lengths; Q <= n
+    const long long units = std::min((long long)n * ((max_k + kThreads - 1) / kThreads), (long long)sm_count() * 16);
+    pr_tail_kernel<<<(int)std::max(1ll, units), kThreads, 0, st>>>(off, nq, (long long)max_k, adaptive_k, positives, precision, recall);
     count_launch();
-    const int cgrid = (int)std::max(1ll, std::min((long long)n / kLongQuery, (long long)sm_count() * 2));
-    eval_cta_kernel<<<cgrid, kCtaThreads, 0, st>>>(a, long_list, long_count);
-    count_launch();
-    return check_cuda(cudaGetLastError(), "retrieval_evaluate");
+    return check_cuda(cudaGetLastError(), "retrieval_pr_curve");
 }

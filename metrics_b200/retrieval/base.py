@@ -125,14 +125,17 @@ class RetrievalMetric(Metric, ABC):
     def _empty_flags(self) -> Tensor:
         return _native.retrieval_evaluate(self._groups(), self._kind)[1]
 
-    def compute(self) -> Tensor:
-        """Per-query values from one evaluation launch over the shared group sort, then empty handling and aggregation."""
-        preds = dim_zero_cat(self.preds)
-        groups = self._groups()
+    def _evaluate(self, groups: "_native.RetrievalGroups") -> "tuple[Tensor, Tensor]":
+        """``(value float32 [Q], empty bool [Q])`` of every query from the sorted groups: one evaluation launch."""
         ideal = None
         if self._kind == _native.RET_NDCG:
             ideal = self._cached("ideal", lambda: _native.retrieval_sort_ideal(groups))
-        value, empty = _native.retrieval_evaluate(groups, self._kind, ideal=ideal, **self._metric_args())
+        return _native.retrieval_evaluate(groups, self._kind, ideal=ideal, **self._metric_args())
+
+    def compute(self) -> Tensor:
+        """Per-query values from one evaluation launch over the shared group sort, then empty handling and aggregation."""
+        preds = dim_zero_cat(self.preds)
+        value, empty = self._evaluate(self._groups())
         action = self.empty_target_action
         if action == "error":
             if bool(empty.any()):
