@@ -304,7 +304,8 @@ MB200_API int mb200_coco_map_accumulate(const int32_t* det_cat, const float* det
  * (multilabel), confusion_matrix.py:119-152 and :477-516 (the 2x2 matrices are [[tn, fp], [fn, tp]]).
  *
  *  preds   : [n_outer, num_labels, inner] contiguous; floating scores (sigmoid applied when ANY value of the call
- *            lies outside [0,1], then `> threshold`) or integer labels compared raw against the target.
+ *            lies outside [0,1], then `> threshold` with the threshold rounded to the score dtype, double -> float ->
+ *            half / bfloat16, as ATen rounds a Python scalar) or integer labels compared raw against the target.
  *  target  : same layout, integer; elements equal to ignore_index are skipped; values outside {0,1} are skipped and
  *            flagged (MB200_FLAG_TARGET_RANGE); integer preds outside {0,1} are flagged (MB200_FLAG_PREDS_RANGE).
  *  counts  : int64 [G][4] += (tp, fp, tn, fn), G = num_labels, or n_outer * num_labels when samplewise != 0.

@@ -73,7 +73,7 @@ struct BinArgs {
     long long n_outer;
     long long num_labels;
     long long inner;
-    float threshold;
+    float threshold;  // rounded to the score dtype, as ATen rounds the reference's scalar (threshold_in_dtype)
     double threshold_d;
     int has_ignore;
     long long ignore_index;
@@ -262,8 +262,9 @@ __global__ void __launch_bounds__(256) bin_count_flat_kernel(BinArgs a) {
 // probabilities, four assuming logits — while the vote itself is taken on the way; a one-warp epilogue kernel adds the set the
 // vote selected to the states.  Counting under "logits" does not evaluate a sigmoid per element: sigmoid(x) > thr is decided
 // by comparing x with a bracket [x_lo, x_hi] around logit(thr) computed on the host in double precision, wide enough to cover
-// the rounding of the float32 sigmoid and of its store in T; only scores INSIDE the bracket (a ~2^-7 .. 2^-20 relative band
-// around the threshold) run the exact arithmetic of `pred_from_value`, so the result is bit-identical to the two-pass kernels.
+// the rounding of the float32 sigmoid and of its store in T; only scores INSIDE the bracket (one spacing of T above the
+// threshold, plus a 2^-20 relative band) run the exact arithmetic of `pred_from_value`, so the result is bit-identical to the
+// two-pass kernels.
 struct BothArgs {
     float x_lo, x_hi;            // outside (x_lo, x_hi): sigmoid(x) > thr is decided by the side; NaN bracket = always exact
     unsigned long long* both;    // [8] zeroed scratch: tp fp tn fn under "probabilities", then under "logits"
@@ -396,6 +397,30 @@ __global__ void __launch_bounds__(256) bin_count_cols_kernel(BinArgs a) {
 
 using namespace mb200;
 
+// The threshold the reference's `preds > threshold` compares a score with: ATen casts the Python float to the score dtype
+// first (double -> float -> half / bfloat16, each round-to-nearest-even), so a float16 score of 0.30004883 is NOT above 0.3.
+static float threshold_in_dtype(double threshold, int dtype) {
+    const float f = (float)threshold;
+    if (dtype == MB200_F16) return __half2float(__float2half_rn(f));
+    if (dtype == MB200_BF16) return __bfloat162float(__float2bfloat16_rn(f));
+    return f;
+}
+
+// the next value above v (finite, >= 0) representable in the score dtype
+static float next_in_dtype(float v, int dtype) {
+    if (dtype == MB200_F16) {
+        __half_raw r = __float2half_rn(v);
+        ++r.x;
+        return __half2float(__half(r));
+    }
+    if (dtype == MB200_BF16) {
+        __nv_bfloat16_raw r = __float2bfloat16_rn(v);
+        ++r.x;
+        return __bfloat162float(__nv_bfloat16(r));
+    }
+    return std::nextafter(v, INFINITY);
+}
+
 static int binary_stat_counts_impl(const void* preds, int preds_dtype, const void* target, int target_dtype, int64_t n_outer,
                                    int64_t num_labels, int64_t inner, double threshold, int has_ignore_index,
                                    int64_t ignore_index, int samplewise, int64_t* counts, uint32_t* flag_scratch,
@@ -412,7 +437,7 @@ static int binary_stat_counts_impl(const void* preds, int preds_dtype, const voi
     BinArgs a;
     a.preds = preds, a.target = target, a.preds_dtype = preds_dtype, a.target_dtype = target_dtype;
     a.n_outer = n_outer, a.num_labels = num_labels, a.inner = inner;
-    a.threshold = (float)threshold, a.threshold_d = threshold;
+    a.threshold = threshold_in_dtype(threshold, preds_dtype), a.threshold_d = threshold;
     a.has_ignore = has_ignore_index, a.ignore_index = ignore_index, a.samplewise = samplewise;
     a.counts = reinterpret_cast<long long*>(counts);
     a.logits = float_preds ? flag_scratch : nullptr;
@@ -434,10 +459,15 @@ static int binary_stat_counts_impl(const void* preds, int preds_dtype, const voi
         BothArgs b;
         b.vote = flag_scratch;
         b.both = reinterpret_cast<unsigned long long*>(flag_scratch + 2);
-        // bracket around logit(threshold): rel. band eps covers the float32 sigmoid's error and its rounding to T
-        const double eps = preds_dtype == MB200_F32 ? 0x1p-20 : (preds_dtype == MB200_F16 ? 0x1p-9 : 0x1p-6);
-        const double lo_p = threshold * (1.0 - eps) - 1e-300, hi_p = threshold * (1.0 + eps) + 1e-300;
-        if (threshold > 1e-6 && hi_p < 1.0 - 1e-6) {
+        // bracket around logit(threshold).  The exact decision compares s = the float32 sigmoid (rounded to T) with the
+        // T-valued a.threshold; it can only flip for s in (thr, up], up the next T value above thr: s <= thr rounds to at
+        // most thr, s >= up to at least up.  The float32 sigmoid is within 2^-21 relative of sigmoid(x) (expf <= 2 ulp,
+        // add and divide 0.5 ulp each) while s is a normal float32, so eps = 2^-20 around [thr, up] holds every score
+        // whose side is in doubt.  up - thr is T's absolute spacing at thr, float16 subnormals included.  A threshold
+        // that rounds to <= 1e-6 or whose band reaches 1 has no bracket: every score runs the exact arithmetic.
+        const double eps = 0x1p-20, thr = a.threshold, up = next_in_dtype(a.threshold, preds_dtype);
+        const double lo_p = thr * (1.0 - eps), hi_p = up * (1.0 + eps);
+        if (thr > 1e-6 && hi_p < 1.0 - 1e-6) {
             const double xl = std::log(lo_p / (1.0 - lo_p)), xh = std::log(hi_p / (1.0 - hi_p));
             b.x_lo = (float)(xl - 1e-5 * (1.0 + std::fabs(xl)));
             b.x_hi = (float)(xh + 1e-5 * (1.0 + std::fabs(xh)));

@@ -1,11 +1,11 @@
 """GPU: the single-pass binary counting kernel (csrc/binary.cu `bin_count_flat_both_kernel`: both outcomes of the logits vote
 counted in one read, sigmoid(x) > thr decided by a host-computed bracket around logit(thr)) is bit-identical to the two-pass
 kernels behind `mb200_binary_stat_counts` (vote pass, then counting with the exact float32 sigmoid of ATen) — in particular
-for scores crowded around the threshold crossing, where the bracket hands over to the exact arithmetic — and to the oracle."""
+for scores crowded around the threshold crossing, where the bracket hands over to the exact arithmetic — and to the
+reference's rule: the score in its own dtype compared with the threshold rounded to that dtype, as ATen rounds the scalar."""
 import ctypes
 import math
 
-import numpy as np
 import pytest
 import torch
 
@@ -28,7 +28,13 @@ def _two_pass(preds, target, threshold, ignore_index):
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float16, torch.bfloat16])
-@pytest.mark.parametrize("threshold", [0.5, 0.1, 0.9, 0.999, 1e-4, 0.0, 1.0, 0.3333333])
+@pytest.mark.parametrize("threshold", [0.5, 0.1, 0.9, 0.999, 1e-4, 0.0, 1.0, 0.3333333,
+                                       # not representable in half precision: bf16(0.3) = 0.30078125, bf16(0.9999) = 1.0
+                                       0.3, 0.7, 0.9999,
+                                       # float16 subnormal range: the spacing (2^-24) exceeds thr * 2^-9
+                                       2e-6, 1.2e-5, 3e-5, 6e-5,
+                                       # rounded to float32 first, these fall on the other side of a half-precision midpoint
+                                       0.5 + 2**-12 + 2**-40, 0.5 + 2**-9 + 2**-40])
 @pytest.mark.parametrize("kind", ["logits", "probs"])
 def test_single_pass_equals_two_pass(dtype, threshold, kind):
     n = 1 << 18
@@ -50,11 +56,10 @@ def test_single_pass_equals_two_pass(dtype, threshold, kind):
         got = _native.binary_stat_counts(x, t, 1, threshold, ignore, False)
         want = _two_pass(x, t, threshold, ignore)
         assert torch.equal(got, want), (got, want)
-    # oracle: float32 sigmoid of the T-rounded score, rounded back to T, compared with the float32 threshold
-    xf = x.float().cpu()
-    if kind == "logits":
-        xf = torch.sigmoid(x).float().cpu()  # ATen CUDA sigmoid == K6 (tests/test_normalize_aten_gpu.py)
-    p = (xf > np.float32(threshold)).long()
+    # oracle: the reference's rule — the score (for logits its float32 sigmoid stored in T) compared in T with the Python
+    # float, which ATen rounds to T first
+    xs = torch.sigmoid(x) if kind == "logits" else x  # ATen CUDA sigmoid == K6 (tests/test_normalize_aten_gpu.py)
+    p = (xs > threshold).long().cpu()
     tt = t.cpu()
     keep = tt != -1
     exp = [int(((p == 1) & (tt == 1) & keep).sum()), int(((p == 1) & (tt == 0) & keep).sum()),
