@@ -35,6 +35,7 @@ from metrics_b200.classification import (  # noqa: F401  (reference __init__.py:
 from metrics_b200.regression import (  # noqa: F401  (reference __init__.py:113-134)
     CriticalSuccessIndex,
     ExplainedVariance,
+    KendallRankCorrCoef,
     KLDivergence,
     LogCoshError,
     MeanAbsoluteError,
@@ -44,6 +45,7 @@ from metrics_b200.regression import (  # noqa: F401  (reference __init__.py:113-
     MinkowskiDistance,
     R2Score,
     RelativeSquaredError,
+    SpearmanCorrCoef,
     SymmetricMeanAbsolutePercentageError,
     TweedieDevianceScore,
     WeightedMeanAbsolutePercentageError,

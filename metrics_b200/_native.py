@@ -155,12 +155,19 @@ RETRIEVAL_SIGNATURES = {
     "mb200_retrieval_pr_curve_scratch_bytes": ("q", "q"),
     "mb200_retrieval_pr_curve": ("i", "ppppqqippppqp"),
 }
+# The rank-correlation entry points (K17) are declared in include/metrics_b200_rankcorr.h, exported from the same library;
+# tests/test_rankcorr_surface.py holds this table to that header.
+RANKCORR_SIGNATURES = {
+    "mb200_rankcorr_scratch_bytes": ("q", "qqi"),
+    "mb200_spearman_corrcoef": ("i", "pipiqqpidpqpp"),
+    "mb200_kendall_rank_corrcoef": ("i", "pipiqqiipippqpp"),
+}
 
 
 def declare_signatures(handle) -> None:
     """Set ``restype`` / ``argtypes`` of every exported function on a loaded library handle."""
     for name, (ret, args) in (*SIGNATURES.items(), *CALIBRATION_SIGNATURES.items(), *SEGMENTATION_SIGNATURES.items(),
-                                *RETRIEVAL_SIGNATURES.items()):
+                                *RETRIEVAL_SIGNATURES.items(), *RANKCORR_SIGNATURES.items()):
         fn = getattr(handle, name)
         fn.restype = _C_TYPES[ret]
         fn.argtypes = [_C_TYPES[a] for a in args]
@@ -1195,3 +1202,81 @@ def retrieval_pr_curve(groups: RetrievalGroups, max_k: int, adaptive_k: bool = F
                                            recall.data_ptr(), empty.data_ptr(), scratch.data_ptr(), nbytes, stream_handle(dev))
     check(rc, "retrieval_pr_curve")
     return precision[:q], recall[:q], empty[:q].bool()
+
+
+# ----------------------------------------------------------------------------------------------------------
+# K17 wrappers (rank correlations, include/metrics_b200_rankcorr.h)
+# ----------------------------------------------------------------------------------------------------------
+RANKCORR_MAX_ROWS = (1 << 30) - 1
+KENDALL_VARIANT = {"a": 0, "b": 1, "c": 2}
+KENDALL_ALTERNATIVE = {None: 0, "two-sided": 1, "less": 2, "greater": 3}
+_RANKABLE = (torch.float32, torch.float16, torch.bfloat16, torch.float64, torch.int32, torch.int64)
+
+
+def rankcorr_scratch_bytes(n: int, d: int, kendall: bool) -> int:
+    """Workspace of one K17 call; raises ValueError from 2^30 rows on (the radix sort counts in 30 bits)."""
+    nbytes = int(lib().mb200_rankcorr_scratch_bytes(int(n), int(d), int(bool(kendall))))
+    if nbytes < 0:
+        raise ValueError(f"metrics_b200: rank correlations support at most 2^30 - 1 = {RANKCORR_MAX_ROWS} rows per column, "
+                         f"got {n} rows x {d} columns.")
+    return nbytes
+
+
+def _rank_columns(x: Tensor) -> Tensor:
+    """``[N]`` or ``[N, d]`` as a contiguous row-major tensor of a dtype the kernel ranks (other integer types and bool
+    are widened to int64, which keeps their order)."""
+    if x.dtype not in _RANKABLE:
+        x = x.to(torch.int64)
+    return x.contiguous()
+
+
+def _rankcorr_launch(preds: Tensor, target: Tensor, kendall: bool):
+    dev = require_cuda(preds, target)
+    n = preds.shape[0] if preds.ndim else 1
+    d = preds.shape[1] if preds.ndim == 2 else 1
+    nbytes = rankcorr_scratch_bytes(n, d, kendall)  # the size guard, before anything is allocated
+    preds, target = _rank_columns(preds), _rank_columns(target)
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    err = torch.zeros(1, dtype=torch.int32, device=dev)
+    return dev, n, d, preds, target, scratch, err
+
+
+def _check_sort_flag(err: Tensor, what: str) -> None:
+    if int(err.item()) & FLAG_SPIN_TIMEOUT:
+        raise NativeLibraryError(f"metrics_b200.{what}: the radix sort's look-back wait expired (results invalid)")
+
+
+def spearman_corrcoef(preds: Tensor, target: Tensor, out_dtype: torch.dtype, eps: float = 1e-6) -> Tensor:
+    """K17: Spearman's rho of every column of ``preds`` / ``target`` (``[N]`` or ``[N, d]``, floating point), ``[d]`` in
+    ``out_dtype`` (a scalar for 1-d inputs).  One host synchronisation: the sort's error flag."""
+    dev, n, d, preds, target, scratch, err = _rankcorr_launch(preds, target, kendall=False)
+    out = torch.empty(d, dtype=out_dtype, device=dev)
+    with on_device(dev):
+        rc = lib().mb200_spearman_corrcoef(preds.data_ptr(), tag(preds), target.data_ptr(), tag(target), n, d, out.data_ptr(),
+                                           tag(out), float(eps), scratch.data_ptr(), scratch.numel(), err.data_ptr(), stream_handle(dev))
+    check(rc, "spearman_corrcoef")
+    _check_sort_flag(err, "spearman_corrcoef")
+    return out.reshape(()) if preds.ndim == 1 else out
+
+
+def kendall_rank_corrcoef(preds: Tensor, target: Tensor, variant: str, alternative: Optional[str]) -> tuple[Tensor, Optional[Tensor]]:
+    """K17: Kendall's tau (``variant`` "a", "b" or "c") of every column and, unless ``alternative`` is None, the p-value of
+    its t-test; ``[d]``, scalars when d == 1.  The p-value is float32, and so is tau except for variant "c", which has the
+    promoted floating dtype of the inputs (as in the reference).  One host synchronisation: the sort's error flag."""
+    tau_dtype = torch.promote_types(preds.dtype, target.dtype) if variant == "c" else torch.float32
+    if not tau_dtype.is_floating_point:
+        tau_dtype = torch.float32
+    dev, n, d, preds, target, scratch, err = _rankcorr_launch(preds, target, kendall=True)
+    tau = torch.empty(d, dtype=tau_dtype, device=dev)
+    p_value = None if alternative is None else torch.empty(d, dtype=torch.float32, device=dev)
+    with on_device(dev):
+        rc = lib().mb200_kendall_rank_corrcoef(preds.data_ptr(), tag(preds), target.data_ptr(), tag(target), n, d,
+                                               KENDALL_VARIANT[variant], KENDALL_ALTERNATIVE[alternative], tau.data_ptr(),
+                                               tag(tau), ptr(p_value), scratch.data_ptr(), scratch.numel(), err.data_ptr(),
+                                               stream_handle(dev))
+    check(rc, "kendall_rank_corrcoef")
+    _check_sort_flag(err, "kendall_rank_corrcoef")
+    if d == 1:
+        tau = tau.reshape(())
+        p_value = None if p_value is None else p_value.reshape(())
+    return tau, p_value

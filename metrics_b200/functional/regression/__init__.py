@@ -16,6 +16,8 @@ from metrics_b200.functional.regression.metrics import (  # noqa: F401
 )
 
 from metrics_b200.functional.regression.kl_divergence import kl_divergence  # noqa: F401,E402
+from metrics_b200.functional.regression.kendall import kendall_rank_corrcoef  # noqa: F401,E402
+from metrics_b200.functional.regression.spearman import spearman_corrcoef  # noqa: F401,E402
 
 # The reference's import paths `<package>.{explained_variance}` are alias submodules that share a name with a function exported
 # above.  Loading a submodule binds it as a package attribute, so load them now and re-bind the functions afterwards: a
