@@ -94,6 +94,19 @@ __device__ __forceinline__ long long load_label(const void* p, int dtype, long l
     }
 }
 
+// `ignore_index` as the reference compares it with labels of this dtype: `target != ignore_index` casts the Python int to
+// the target's dtype first (two's complement wrap), so with uint8 targets 257 is 1 and -1 is 255, with int8 255 is -1.
+// int64 keeps the value; a bool target promotes the comparison to int64, so it is not wrapped either.
+inline long long label_ignore_index(long long v, int dtype) {
+    switch (dtype) {
+        case MB200_I32: return (int32_t)(uint32_t)v;
+        case MB200_I16: return (int16_t)(uint16_t)v;
+        case MB200_I8: return (int8_t)(uint8_t)v;
+        case MB200_U8: return (uint8_t)v;
+        default: return v;
+    }
+}
+
 __device__ __forceinline__ void red_add_u64(long long* addr, unsigned long long v) {
     atomicAdd(reinterpret_cast<unsigned long long*>(addr), v);
 }

@@ -506,7 +506,7 @@ extern "C" int mb200_multiclass_confmat_update(const void* preds, int preds_dtyp
                   (long long)num_classes);
     if (n_outer * inner == 0) return 0;
     RowArgs a{preds, target, target_dtype, n_outer, (int)num_classes, inner, has_ignore_index,
-              ignore_index, err_flag};
+              label_ignore_index(ignore_index, target_dtype), err_flag};
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const bool priv = num_classes * num_classes <= 4096 && n_outer * inner >= 4096;
     if (priv) {
@@ -528,7 +528,7 @@ extern "C" int mb200_multiclass_stat_scores_update(const void* preds, int preds_
     MB200_REQUIRE(tp && fp && tn && fn && workspace, "state / workspace pointer is NULL");
     if (n_outer * inner == 0) return 0;
     RowArgs a{preds, target, target_dtype, n_outer, (int)num_classes, inner, has_ignore_index,
-              ignore_index, err_flag};
+              label_ignore_index(ignore_index, target_dtype), err_flag};
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     // Shared-memory privatisation pays when many rows hit few class bins (L2 atomics on a handful of addresses
     // serialise).  With hundreds of classes the ~2 REDs per row spread over 3C L2-resident words cost nothing, while
@@ -578,7 +578,8 @@ extern "C" int mb200_multiclass_stat_scores_topk_update(const void* preds, int p
     MB200_REQUIRE(tp && fp && tn && fn && workspace, "state / workspace pointer is NULL");
     MB200_REQUIRE(top_k >= 1 && top_k <= num_classes, "top_k must be in [1, num_classes]");
     if (n == 0) return 0;
-    RowArgs a{preds, target, target_dtype, n, (int)num_classes, 1, has_ignore_index, ignore_index, err_flag};
+    RowArgs a{preds, target, target_dtype, n, (int)num_classes, 1, has_ignore_index,
+              label_ignore_index(ignore_index, target_dtype), err_flag};
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     StatsSink<false> s{(long long*)tp, (long long*)fp, (long long*)tn, (long long*)fn, (long long*)workspace,
                        (int)num_classes, 0};
@@ -594,7 +595,8 @@ extern "C" int mb200_multiclass_stat_scores_samplewise(const void* preds, int pr
     if (int rc = validate_common(preds, target, target_dtype, n_outer, num_classes, inner, true)) return rc;
     MB200_REQUIRE(counts && n_valid, "NULL pointer");
     if (n_outer * inner == 0) return 0;
-    RowArgs a{preds, target, target_dtype, n_outer, (int)num_classes, inner, has_ignore_index, ignore_index, err_flag};
+    RowArgs a{preds, target, target_dtype, n_outer, (int)num_classes, inner, has_ignore_index,
+              label_ignore_index(ignore_index, target_dtype), err_flag};
     SamplewiseSink s{(long long*)counts, (long long*)n_valid, n_outer, inner, (int)num_classes};
     return dispatch_rows(preds_dtype, preds_has_class_dim, a, s, 0, reinterpret_cast<cudaStream_t>(stream));
 }
