@@ -75,13 +75,14 @@ def lib() -> ctypes.CDLL:
     return _lib
 
 
-# Return / argument types of every entry point of include/metrics_b200.h, one letter per C type (tests/test_native_abi.py
-# re-derives this table from the header and fails when they drift apart).  Declaring them lets ctypes convert plain Python
+# Return / argument types of every entry point of include/metrics_b200*.h, one letter per C type (tests/test_abi.py
+# re-derives this table from the headers and fails when they drift apart).  Declaring them lets ctypes convert plain Python
 # ints / floats / None itself — no `c_void_p` / `c_int64` object per argument on the launch path, a large share of the host
 # time of a small `update()` — and makes a wrong argument count or kind a TypeError instead of a silent truncation.
 _C_TYPES = {"i": ctypes.c_int, "q": ctypes.c_int64, "Q": ctypes.c_uint64, "d": ctypes.c_double, "p": ctypes.c_void_p,
             "s": ctypes.c_char_p}
 SIGNATURES = {
+    # include/metrics_b200.h
     "mb200_abi_version": ("i", ""),
     "mb200_last_error": ("s", ""),
     "mb200_launch_count": ("Q", ""),
@@ -126,24 +127,15 @@ SIGNATURES = {
     "mb200_peer_pack_keys_put": ("i", "piqqqiqqpqp"),
     "mb200_peer_put_all": ("i", "pqpqip"),
     "mb200_peer_reduce_put_i64": ("i", "pqqqiiip"),
-}
-# The calibration-error entry points (K14) are declared in the companion header include/metrics_b200_calibration.h and
-# exported from the same library; tests/test_calibration_abi.py holds this table to that header.
-CALIBRATION_SIGNATURES = {
+    # include/metrics_b200_calibration.h
     "mb200_calibration_scratch_bytes": ("q", "q"),
     "mb200_calibration_top_label": ("i", "pipiqqiqpppqpp"),
     "mb200_calibration_bin_scratch_bytes": ("q", "qq"),
     "mb200_calibration_bin_sums": ("i", "pipiqpqppppqp"),
-}
-# The segmentation overlap-count entry point (K15) is declared in include/metrics_b200_segmentation.h, exported from the same
-# library; tests/test_segmentation_abi.py holds this table to that header.
-SEGMENTATION_SIGNATURES = {
+    # include/metrics_b200_segmentation.h
     "mb200_segmentation_scratch_bytes": ("q", "qqqiiii"),
     "mb200_segmentation_overlap_counts": ("i", "pipiqqqiiqqiippqpp"),
-}
-# The retrieval entry points (K16) are declared in include/metrics_b200_retrieval.h, exported from the same library;
-# tests/test_retrieval_abi.py holds this table to that header.
-RETRIEVAL_SIGNATURES = {
+    # include/metrics_b200_retrieval.h
     "mb200_retrieval_index_range": ("i", "pqpp"),
     "mb200_retrieval_sort_scratch_bytes": ("q", "qi"),
     "mb200_retrieval_sort": ("i", "pppiqqqpppppqp"),
@@ -154,10 +146,7 @@ RETRIEVAL_SIGNATURES = {
     "mb200_retrieval_auroc": ("i", "ppppqqdpppqp"),
     "mb200_retrieval_pr_curve_scratch_bytes": ("q", "q"),
     "mb200_retrieval_pr_curve": ("i", "ppppqqippppqp"),
-}
-# The rank-correlation entry points (K17) are declared in include/metrics_b200_rankcorr.h, exported from the same library;
-# tests/test_rankcorr_surface.py holds this table to that header.
-RANKCORR_SIGNATURES = {
+    # include/metrics_b200_rankcorr.h
     "mb200_rankcorr_scratch_bytes": ("q", "qqi"),
     "mb200_spearman_corrcoef": ("i", "pipiqqpidpqpp"),
     "mb200_kendall_rank_corrcoef": ("i", "pipiqqiipippqpp"),
@@ -166,8 +155,7 @@ RANKCORR_SIGNATURES = {
 
 def declare_signatures(handle) -> None:
     """Set ``restype`` / ``argtypes`` of every exported function on a loaded library handle."""
-    for name, (ret, args) in (*SIGNATURES.items(), *CALIBRATION_SIGNATURES.items(), *SEGMENTATION_SIGNATURES.items(),
-                                *RETRIEVAL_SIGNATURES.items(), *RANKCORR_SIGNATURES.items()):
+    for name, (ret, args) in SIGNATURES.items():
         fn = getattr(handle, name)
         fn.restype = _C_TYPES[ret]
         fn.argtypes = [_C_TYPES[a] for a in args]

@@ -1,33 +1,9 @@
-"""CPU: the C-ABI shared library loads and exports every symbol declared in include/metrics_b200.h."""
-import ctypes
+"""CPU: the kernel wrappers refuse host tensors, product code stays clear of the oracle, and the threshold sortedness cache
+tells tensors apart.  The C-ABI itself is checked in tests/test_abi.py."""
 import os
 import re
 
 from tests.conftest import ROOT
-
-
-def _declared_symbols():
-    text = open(os.path.join(ROOT, "include", "metrics_b200.h")).read()
-    return sorted(set(re.findall(r"MB200_API[^;(]*?\b(mb200_\w+)\s*\(", text)))
-
-
-def test_library_exports_every_declared_symbol():
-    from metrics_b200 import _native
-
-    assert os.path.exists(_native.lib_path()), "build the extension first: python -c 'import __graft_entry__ as g; g.build()'"
-    handle = ctypes.CDLL(_native.lib_path())
-    names = _declared_symbols()
-    assert len(names) >= 6
-    missing = [n for n in names if not hasattr(handle, n)]
-    assert not missing, f"symbols declared in the header but not exported: {missing}"
-
-
-def test_abi_version_and_error_string():
-    from metrics_b200 import _native
-
-    lib = _native.lib()
-    assert lib.mb200_abi_version() == 1
-    assert isinstance(lib.mb200_last_error(), bytes)
 
 
 def test_cpu_tensors_are_rejected_loudly():
@@ -51,217 +27,6 @@ def test_product_never_imports_the_oracle():
                 if re.search(r"^\s*(from|import)\s+(oracle|tests)\b", src, re.M) or "cpu_kernels" in src:
                     bad.append(os.path.join(dirpath, f))
     assert not bad, f"product code must not import oracle/ or the test stand-ins: {bad}"
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# ctypes signatures: the table in _native.py vs the header, and every wrapper's call vs the table
-# ---------------------------------------------------------------------------------------------------------------------
-def _header_signatures():
-    """{name: (return letter, argument letters)} parsed from include/metrics_b200.h (p void*/T*, i int, q int64_t,
-    Q uint64_t, d double, s const char*)."""
-    text = open(os.path.join(ROOT, "include", "metrics_b200.h")).read()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    text = re.sub(r"//[^\n]*", "", text)
-
-    def letter(ctype: str) -> str:
-        ctype = ctype.strip()
-        if "char" in ctype and "*" in ctype:
-            return "s"
-        if "*" in ctype:
-            return "p"
-        return {"int": "i", "int64_t": "q", "uint64_t": "Q", "double": "d"}[ctype.replace("const", "").split()[0]]
-
-    out = {}
-    for ret, name, args in re.findall(r"MB200_API\s+([\w\s\*]+?)\s*(mb200_\w+)\s*\(([^)]*)\)\s*;", text):
-        params = [a.strip() for a in " ".join(args.split()).split(",")]
-        params = [] if params == ["void"] else params
-        out[name] = (letter(ret), "".join(letter(p.rsplit(" ", 1)[0]) for p in params))
-    return out
-
-
-def test_signature_table_matches_the_header():
-    from metrics_b200 import _native
-
-    assert _native.SIGNATURES == _header_signatures()
-    handle = _native.lib()
-    for name, (ret, args) in _native.SIGNATURES.items():
-        fn = getattr(handle, name)
-        assert fn.restype is _native._C_TYPES[ret] and len(fn.argtypes) == len(args), name
-
-
-class _RecordingLibrary:
-    """Stands in for the loaded .so on a box without a GPU: every entry point is a REAL ctypes function pointer with the
-    declared signature (a CFUNCTYPE around a Python callback), so a wrapper that passes the wrong number or kind of
-    arguments fails here exactly as it would against the library.  The callbacks do nothing and report success."""
-
-    def __init__(self, native):
-        self.calls = {}
-        self._keep = []
-        for name, (ret, args) in native.SIGNATURES.items():
-            proto = ctypes.CFUNCTYPE(native._C_TYPES[ret], *[native._C_TYPES[a] for a in args])
-
-            def callback(*values, _name=name, _ret=ret):
-                self.calls.setdefault(_name, []).append(values)
-                if _name.endswith(("_bytes", "_doubles", "_words")):
-                    return 256
-                if _name == "mb200_regression_num_sums":
-                    return 4
-                return b"" if _ret == "s" else 0
-
-            fn = proto(callback)
-            self._keep.append(fn)
-            setattr(self, name, fn)
-
-
-def test_every_kernel_wrapper_calls_the_abi_as_declared(monkeypatch):
-    """Drive each wrapper of `_native.py` once (CPU tensors, device checks patched out, library replaced by
-    `_RecordingLibrary`): argument count and C types must match include/metrics_b200.h, pointers must be non-NULL where a
-    tensor was passed, and the stream handle must arrive as the last argument."""
-    import torch
-
-    from metrics_b200 import _native
-
-    fake = _RecordingLibrary(_native)
-    cpu = torch.device("cpu")
-    monkeypatch.setattr(_native, "lib", lambda: fake)
-    monkeypatch.setattr(_native, "require_cuda", lambda *t: cpu)
-    monkeypatch.setattr(_native, "on_device", lambda d: _native._NOOP)
-    monkeypatch.setattr(_native, "stream_handle", lambda d: 0xABCD)
-    monkeypatch.setattr(_native, "_flag_words", {})
-
-    n, c = 16, 3
-    scores, labels = torch.rand(n, c), torch.randint(c, (n,))
-    i64 = lambda *shape: torch.zeros(*shape, dtype=torch.int64)  # noqa: E731
-    flag = torch.zeros(1, dtype=torch.int32)
-    _native.multiclass_confmat_update_(i64(c, c), scores, labels, c, 1, flag)
-    _native.multiclass_confmat_update_(i64(c, c), labels, labels, c, None, None)
-    _native.multiclass_stat_scores_update_(i64(c), i64(c), i64(c), i64(c), i64(3 * c + 2), scores, labels, c, None, False, flag)
-    _native.multiclass_stats_softmax_update_(i64(c), i64(c), i64(c), i64(c), i64(3 * c + 2), scores, labels, c, False, flag)
-    _native.multiclass_stat_scores_topk_update_(i64(c), i64(c), i64(c), i64(c), i64(3 * c + 2), scores, labels, c, 2, None, None)
-    _native.multiclass_stat_scores_samplewise(scores.reshape(4, c, 4), labels.reshape(4, 4), c, None, flag)
-    _native.argmax_rows(scores)
-    _native.sigmoid_if_logits(scores[:, 0])
-    _native.sigmoid_if_logits(torch.rand(40000))
-    _native.softmax_if_logits(scores)
-    _native.softmax_if_logits(scores.double())
-    _native.curve_evaluate(scores[:, 0], labels.clamp(max=1), 1, 1, want_curve=True)
-    _native.curve_evaluate(scores, labels, c, unit_range=False)
-    keys = _native.curve_pack_keys(scores, c)
-    _native.curve_evaluate_keys(keys, labels, 0)
-    _native.curve_evaluate_keys(keys, labels, 0, nonneg=True)
-    _native.curve_evaluate_multilabel(scores, torch.randint(2, (n, c)), c, ignore_index=-1, want_curve=True)
-    _native.binary_stat_counts(scores, torch.randint(2, (n, c)), c, 0.5, None, False, None, flag)
-    _native.binary_stat_counts(scores[:, 0], torch.randint(2, (n,)), 1, 0.5, 0, True)
-    _native.regression_sums(scores[:, 0], scores[:, 1], 0)
-    _native.binned_curve_update(scores[:, 0], labels.clamp(max=1), torch.linspace(0, 1, 5), 1)
-    _native.binned_curve_update(scores, torch.randint(2, (n, c)), torch.linspace(0, 1, 5), c, multilabel=True)
-    boxes = torch.rand(4, 4)
-    _native.coco_map_evaluate(boxes, torch.rand(4), torch.zeros(4, dtype=torch.long), [2, 2], boxes, torch.zeros(4, dtype=torch.long),
-                              torch.zeros(4, dtype=torch.uint8), torch.ones(4), [2, 2], torch.zeros(1, dtype=torch.long), False,
-                              [0.5, 0.75], [0.0, 0.5, 1.0], [1, 10, 100])
-    _native.curve_weighted_clf_curve(scores[:, 0].double(), labels.clamp(max=1), torch.rand(n), 1)
-    # K10: the peer-memory exchange wrappers live on the workspace object (metrics_b200/peer.py); drive them on a bare one
-    from metrics_b200 import peer
-
-    ws = peer.PeerWorkspace.__new__(peer.PeerWorkspace)
-    ws.device, ws.nbytes, ws.world, ws.rank, ws.table = cpu, 1 << 20, 2, 0, 0x1000
-    ws.put_all(labels, 256)
-    ws.pack_keys_put(scores, 2, 2 * n, n, 0)
-    ws.reduce_put_i64(0, 4096, 100, 0)
-    recs, npig, _ = _native.coco_map_match(boxes, torch.rand(4), torch.zeros(4, dtype=torch.long), [2, 2], boxes,
-                                           torch.zeros(4, dtype=torch.long), torch.zeros(4, dtype=torch.uint8), torch.ones(4), [2, 2],
-                                           torch.zeros(1, dtype=torch.long), [0.5, 0.75], 100)
-    _native.coco_map_accumulate(recs[0], torch.rand(4), recs[1], recs[2], recs[3], npig, 1, 0, 1, 2, [0.0, 0.5, 1.0], [1, 10, 100])
-    _native.kl_divergence_rows(scores, scores + 1.0, False)  # K13
-    # K12: instance masks
-    words, area = _native.mask_pack_bits(torch.rand(4, 5, 7) > 0.5)
-    _native.mask_pack_entry(torch.rand(4, 5, 7) > 0.5)
-    off = torch.arange(4, dtype=torch.int64) * words.shape[1]
-    img_off = torch.tensor([0, 2, 4], dtype=torch.int32)
-    inter = _native.mask_pair_intersections(words.reshape(-1), off, words.reshape(-1), off, img_off, img_off,
-                                            torch.tensor([2, 2], dtype=torch.int32), torch.zeros(4, dtype=torch.long),
-                                            torch.zeros(4, dtype=torch.long), False, torch.tensor([0, 4]), 8, 4)
-    _native.coco_map_match(boxes, torch.rand(4), torch.zeros(4, dtype=torch.long), [2, 2], boxes, torch.zeros(4, dtype=torch.long),
-                           torch.zeros(4, dtype=torch.uint8), torch.ones(4), [2, 2], torch.zeros(1, dtype=torch.long), [0.5, 0.75], 100,
-                           micro=True, masks={"pair_inter": inter, "pair_off": torch.tensor([0, 4]), "det_area": area.double(),
-                                              "gt_area": area.double()}, gt_area_exact=True)
-    assert _native.launch_count() == 0
-
-    # (`mb200_regression_num_sums` is a query for C callers; the Python mirror knows the layout of each op's sums)
-    kernels = {k for k in _native.SIGNATURES if k not in ("mb200_abi_version", "mb200_last_error", "mb200_regression_num_sums",
-                                                          "mb200_curve_workspace_bytes", "mb200_binary_stat_counts")}
-    never_called = sorted(kernels - set(fake.calls))
-    assert not never_called, f"no wrapper exercised: {never_called}"
-    for name, calls in fake.calls.items():
-        args = _native.SIGNATURES[name][1]
-        for values in calls:
-            assert len(values) == len(args)
-            if args.endswith("p") and name not in ("mb200_last_error",) and "workspace" not in name:
-                assert values[-1] == 0xABCD, f"{name}: stream handle is not the last argument"
-            assert not args or args[0] != "p" or values[0] not in (None, 0), f"{name}: first pointer is NULL"
-    # optional pointers really arrive as NULL, required ones as addresses
-    with_flag, without_flag = fake.calls["mb200_multiclass_confmat_update"]
-    assert with_flag[11] not in (None, 0) and without_flag[11] in (None, 0)
-    assert with_flag[8] == 1 and with_flag[9] == 1 and without_flag[8] == 0
-    counts_call = fake.calls["mb200_binary_stat_counts_scratch"][0]
-    assert counts_call[7] == 0.5 and isinstance(counts_call[7], float)
-
-
-def test_binding_and_header_agree_on_the_abi_version():
-    from metrics_b200 import _native
-
-    text = open(os.path.join(ROOT, "include", "metrics_b200.h")).read()
-    assert int(re.search(r"#define\s+MB200_ABI_VERSION\s+(\d+)", text).group(1)) == _native.ABI_VERSION
-    assert _native.lib().mb200_abi_version() == _native.ABI_VERSION
-
-
-def test_real_library_accepts_every_wrappers_arguments_up_to_the_first_cuda_call(monkeypatch):
-    """GPU-less boxes only.  Each wrapper is called against the REAL `.so` with host tensors (device checks patched out):
-    ctypes conversion, the library's own argument validation (`MB200_REQUIRE`) and its host-side set-up must all pass, so the
-    first failure has to be a CUDA runtime error (code -2, no driver) — never an argument error (-1 / ValueError / TypeError)."""
-    import pytest
-    import torch
-
-    if torch.cuda.is_available():
-        pytest.skip("a CUDA device is present: host pointers must not reach the kernels")
-    from metrics_b200 import _native
-
-    cpu = torch.device("cpu")
-    monkeypatch.setattr(_native, "require_cuda", lambda *t: cpu)
-    monkeypatch.setattr(_native, "on_device", lambda d: _native._NOOP)
-    monkeypatch.setattr(_native, "stream_handle", lambda d: 0)
-    monkeypatch.setattr(_native, "_flag_words", {})
-    n, c = 16, 3
-    scores, labels = torch.rand(n, c), torch.randint(c, (n,))
-    i64 = lambda *shape: torch.zeros(*shape, dtype=torch.int64)  # noqa: E731
-    flag = torch.zeros(1, dtype=torch.int32)
-    boxes = torch.rand(4, 4)
-    calls = {
-        "confmat": lambda: _native.multiclass_confmat_update_(i64(c, c), scores, labels, c, 1, flag),
-        "stat_scores": lambda: _native.multiclass_stat_scores_update_(i64(c), i64(c), i64(c), i64(c), i64(3 * c + 2), scores, labels, c, None, True, None),
-        "topk": lambda: _native.multiclass_stat_scores_topk_update_(i64(c), i64(c), i64(c), i64(c), i64(3 * c + 2), scores, labels, c, 2, None, None),
-        "samplewise": lambda: _native.multiclass_stat_scores_samplewise(scores.reshape(4, c, 4), labels.reshape(4, 4), c, None, flag),
-        "argmax": lambda: _native.argmax_rows(scores),
-        "sigmoid": lambda: _native.sigmoid_if_logits(scores[:, 0]),
-        "softmax": lambda: _native.softmax_if_logits(scores),
-        "curve": lambda: _native.curve_evaluate(scores[:, 0], labels.clamp(max=1), 1, 1, want_curve=True),
-        "curve_ovr": lambda: _native.curve_evaluate(scores, labels, c),
-        "pack_keys": lambda: _native.curve_pack_keys(scores, c),
-        "curve_multilabel": lambda: _native.curve_evaluate_multilabel(scores, torch.randint(2, (n, c)), c, ignore_index=-1),
-        "binary_counts": lambda: _native.binary_stat_counts(scores, torch.randint(2, (n, c)), c, 0.5, None, False, None, flag),
-        "regression": lambda: _native.regression_sums(scores[:, 0], scores[:, 1], _native.REG_MSE),
-        "regression_columns": lambda: _native.regression_sums(scores, scores, _native.REG_R2, c),
-        "tweedie": lambda: _native.regression_sums(scores[:, 0] + 0.1, scores[:, 1] + 0.1, _native.REG_TWEEDIE, 1, 1.5),
-        "binned": lambda: _native.binned_curve_update(scores[:, 0], labels.clamp(max=1), torch.linspace(0, 1, 5), 1),
-        "binned_multilabel": lambda: _native.binned_curve_update(scores, torch.randint(2, (n, c)), torch.linspace(0, 1, 5), c, multilabel=True),
-        "coco": lambda: _native.coco_map_evaluate(boxes, torch.rand(4), torch.zeros(4, dtype=torch.long), [2, 2], boxes,
-                                                  torch.zeros(4, dtype=torch.long), torch.zeros(4, dtype=torch.uint8), torch.ones(4), [2, 2],
-                                                  torch.zeros(1, dtype=torch.long), False, [0.5, 0.75], [0.0, 0.5, 1.0], [1, 10, 100]),
-    }
-    for name, call in calls.items():
-        with pytest.raises(_native.NativeLibraryError, match=r"\(code -2\): CUDA error") as info:
-            call()
-        assert "CUDA" in str(info.value), name
 
 
 def test_threshold_sortedness_is_not_shared_between_tensors_at_one_address():

@@ -1,42 +1,7 @@
-"""CPU: the retrieval C-ABI (include/metrics_b200_retrieval.h) and its ctypes table `_native.RETRIEVAL_SIGNATURES`, checked
-the way tests/test_segmentation_abi.py checks the segmentation header; the size guard; tag rejection before any launch."""
-import ctypes
-import os
-import re
-
+"""CPU: the retrieval C-ABI (include/metrics_b200_retrieval.h): the size guard; tag rejection before any launch; CPU tensors
+rejected.  Its signatures and constants are checked in tests/test_abi.py."""
 import pytest
 import torch
-
-from tests.conftest import ROOT
-from tests.test_calibration_abi import _letter
-
-HEADER = os.path.join(ROOT, "include", "metrics_b200_retrieval.h")
-
-
-def _header_signatures():
-    text = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
-    out = {}
-    for ret, name, args in re.findall(r"MB200_API\s+([\w\s\*]+?)\s*(mb200_\w+)\s*\(([^)]*)\)\s*;", text):
-        params = [a.strip() for a in " ".join(args.split()).split(",")]
-        out[name] = (_letter(ret), "".join(_letter(p.rsplit(" ", 1)[0]) for p in params))
-    return out
-
-
-def test_table_matches_the_header_and_the_library_exports_it():
-    from metrics_b200 import _native
-
-    assert '#include "metrics_b200.h"' in open(HEADER).read()
-    assert _native.RETRIEVAL_SIGNATURES == _header_signatures()
-    main = open(os.path.join(ROOT, "include", "metrics_b200.h")).read()
-    assert not set(_header_signatures()) & set(re.findall(r"MB200_API[^;(]*?\b(mb200_\w+)\s*\(", main))
-    raw = ctypes.CDLL(_native.lib_path())
-    assert all(hasattr(raw, n) for n in _native.RETRIEVAL_SIGNATURES)
-    for name, (ret, args) in _native.RETRIEVAL_SIGNATURES.items():
-        fn = getattr(_native.lib(), name)
-        assert fn.restype is _native._C_TYPES[ret] and len(fn.argtypes) == len(args), name
-    kinds = dict(re.findall(r"#define MB200_RET_(\w+) (\d+)\n", open(HEADER).read()))
-    assert [int(kinds[k]) for k in ("AP", "RR", "PRECISION", "RECALL", "HIT_RATE", "FALL_OUT", "R_PRECISION", "NDCG")] == list(range(8))
-    assert _native.lib().mb200_abi_version() == 1
 
 
 def test_size_guard_is_the_scratch_query():
