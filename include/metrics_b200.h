@@ -79,10 +79,8 @@ MB200_API uint64_t mb200_launch_count(void);
  *  err_flag     : optional uint32 device word (may be NULL); MB200_FLAG_* bits are OR-ed in.  Rows with an
  *                 out-of-range label are skipped (the reference raises from bincount/reshape instead).
  * argmax semantics == torch.argmax: first index of the maximum, NaN is maximal (first NaN wins), -0 == +0.
- * Launch behaviour (environment, read once): MB200_ROWS_OVERLAP = 1 (default) launches with programmatic stream
- * serialization and waits for the previous grid of the stream before the first input load (always correct; hides the
- * launch gap between back-to-back updates), 0 = plain launches, 2 = no wait (consecutive updates overlap drain and
- * ramp-up; only valid if the inputs were complete before the previous kernel of the stream started).
+ * The launch uses programmatic stream serialization and waits for the previous grid of the stream before its first
+ * input load.
  * ------------------------------------------------------------------------------------------------ */
 MB200_API int mb200_multiclass_confmat_update(const void* preds, int preds_dtype, int preds_has_class_dim,
                                     const void* target, int target_dtype, int64_t n_outer,

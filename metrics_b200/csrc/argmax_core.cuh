@@ -118,10 +118,6 @@ struct GlobalVecLoader {  // streaming 16-byte loads straight from HBM (consumed
     const uint4* __restrict__ base;
     __device__ __forceinline__ uint4 operator()(int vi) const { return ld_stream16(base + vi); }
 };
-struct SharedVecLoader {  // 16-byte loads from a row staged in shared memory by the bulk-copy engine
-    const uint4* base;
-    __device__ __forceinline__ uint4 operator()(int vi) const { return base[vi]; }
-};
 
 // Vector slots past the end of the row re-read the row's LAST vector (index clamp) instead of being predicated off:
 // duplicates cannot change the maximum, and a duplicate sits in a later slot than the original, so the REDUX.MIN over

@@ -12,9 +12,6 @@
 // holding that maximum (torch.argmax tie rule) — again one REDUX.  Lane 0 then commits one 64-bit RED to
 // the L2-resident state.  No intermediate (argmax vector, t*C+p, C*C bins) ever touches HBM, so the
 // algorithmic traffic is the logits read itself.
-#include <stdlib.h>
-#include <string.h>
-
 #include "argmax_core.cuh"
 #include "common.cuh"
 #include "sinks.cuh"
@@ -34,7 +31,6 @@ struct RowArgs {
     int has_ignore;
     long long ignore_index;
     unsigned* err;
-    int pdl_wait = 1;  // overlapped launches: wait for the previous grid's memory before the first input load
 };
 
 template <bool kI64>
@@ -58,7 +54,7 @@ constexpr int kRowThreads = 256;
 // (1) aligned path: warp per row, 16-byte streaming vector loads from global memory.  The label of the warp's NEXT
 // row is requested before the current row is reduced, so label latency never sits in front of the row loads.
 // With >= 4 resident CTAs/SM the reduction is meant to hide behind the HBM stream; tools/confmat_sweep.cu times this loop
-// against a read-only streaming probe over the same 131 MB and against a TMA/bulk-copy ring (1b).
+// against a read-only streaming probe over the same 131 MB (DESIGN.md §K1 lists the alternatives that measured slower).
 template <typename T, typename Sink, bool kI64>
 __global__ void __launch_bounds__(kRowThreads) rows_vec_kernel(RowArgs a, Sink sink) {
     // Let the next update's grid (launched with programmatic stream serialization, see launch_overlapped) start filling
@@ -69,7 +65,7 @@ __global__ void __launch_bounds__(kRowThreads) rows_vec_kernel(RowArgs a, Sink s
         // grid's memory (it may be the producer of our inputs, triggering its dependents early) is only guaranteed
         // visible after griddepcontrol.wait, so no input is touched before it.  (Prefetching the first rows into L2
         // ahead of the wait was measured and is slower.)
-        if (a.pdl_wait) asm volatile("griddepcontrol.wait;" ::: "memory");
+        asm volatile("griddepcontrol.wait;" ::: "memory");
     }
     sink.block_init();
     typename Sink::Local loc;
@@ -91,122 +87,6 @@ __global__ void __launch_bounds__(kRowThreads) rows_vec_kernel(RowArgs a, Sink s
         const GlobalVecLoader load{reinterpret_cast<const uint4*>(preds + (size_t)r * a.C)};
         const int p = warp_row_argmax_vec<T>(load, nvec, lane);
         if (lane == 0) sink.row(loc, r, t, p);
-    }
-    sink.finish(loc);
-}
-
-// (1b) aligned path, bulk-copy pipeline: one producer thread streams tiles of kRows whole rows into a shared-memory
-// ring with `cp.async.bulk` (1-D TMA, completion counted on an mbarrier); kRows consumer warps each reduce one staged
-// row per tile.  HBM requests stay in flight for the whole ring depth and cost no registers.
-constexpr int kBulkMaxStages = 8;
-
-__device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(unsigned long long* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long* bar, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_LOOP:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra DONE;\n"
-        "bra WAIT_LOOP;\n"
-        "DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, unsigned bytes,
-                                         unsigned long long* bar) {
-    asm volatile(
-        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-            smem_u32(dst_smem)),
-        "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
-        : "memory");
-}
-
-template <typename T, typename Sink, bool kI64, int kRows>
-__global__ void __launch_bounds__((kRows + 1) * 32, 1) rows_bulk_kernel(RowArgs a, Sink sink, int stages) {
-    extern __shared__ __align__(128) unsigned char bulk_smem[];
-    __shared__ __align__(8) unsigned long long full_bar[kBulkMaxStages];
-    __shared__ __align__(8) unsigned long long empty_bar[kBulkMaxStages];
-    typename Sink::Local loc;
-    sink.init(loc);
-    const int lane = threadIdx.x & 31;
-    const int warp = threadIdx.x >> 5;
-    const unsigned row_bytes = (unsigned)a.C * (unsigned)sizeof(T);
-    const unsigned stage_bytes = row_bytes * kRows;
-    const int nvec = (int)(row_bytes >> 4);
-    const int n = (int)a.n_outer;
-    const int n_tiles = (n + kRows - 1) / kRows;
-    const unsigned char* __restrict__ gbase = reinterpret_cast<const unsigned char*>(a.preds);
-    constexpr bool kLabels = Sink::kNeedsTarget;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < stages; ++s) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], kRows);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-
-    if (warp == kRows) {
-        // ===== producer: one elected lane keeps the ring full =====
-        if (lane == 0) {
-            int s = 0;
-            unsigned phase = 0;
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                mbar_wait(&empty_bar[s], phase ^ 1u);  // first lap: passes immediately
-                const int row0 = tile * kRows;
-                const int rows = min(kRows, n - row0);
-                const unsigned bytes = (unsigned)rows * row_bytes;
-                mbar_expect_tx(&full_bar[s], bytes);
-                bulk_g2s(bulk_smem + (size_t)s * stage_bytes, gbase + (size_t)row0 * row_bytes, bytes, &full_bar[s]);
-                if (++s == stages) {
-                    s = 0;
-                    phase ^= 1u;
-                }
-            }
-        }
-    } else {
-        // ===== consumers: warp w reduces row w of every tile; labels are fetched one tile ahead =====
-        int s = 0;
-        unsigned phase = 0;
-        int tile = blockIdx.x;
-        long long t_next = 0;
-        if (kLabels && tile < n_tiles && tile * kRows + warp < n) t_next = fetch_label<kI64>(a, tile * kRows + warp);
-        for (; tile < n_tiles; tile += gridDim.x) {
-            const int r = tile * kRows + warp;
-            const long long t = t_next;
-            const int rn = (tile + (int)gridDim.x) * kRows + warp;
-            if (kLabels && rn < n) t_next = fetch_label<kI64>(a, rn);
-            mbar_wait(&full_bar[s], phase);
-            int p = 0;
-            const bool live = r < n && (!kLabels || admit_label(a, t, lane == 0));
-            if (live) {
-                const SharedVecLoader load{
-                    reinterpret_cast<const uint4*>(bulk_smem + (size_t)s * stage_bytes + (size_t)warp * row_bytes)};
-                p = warp_row_argmax_vec<T>(load, nvec, lane);
-            }
-            __syncwarp();
-            if (lane == 0) {
-                mbar_arrive(&empty_bar[s]);  // this warp's row of the stage now lives in registers / is reduced
-                if (live) sink.row(loc, r, t, p);
-            }
-            if (++s == stages) {
-                s = 0;
-                phase ^= 1u;
-            }
-        }
     }
     sink.finish(loc);
 }
@@ -319,30 +199,6 @@ static inline int grid_for(long long work_items, int items_per_block, int max_bl
     return (int)g;
 }
 
-// Path override for A/B measurements: MB200_ROWS_PATH=vec|bulk (default vec: it measured faster, see (1)).
-static int rows_path_override() {
-    static int cached = -1;
-    if (cached < 0) {
-        const char* e = getenv("MB200_ROWS_PATH");
-        cached = (e && e[0] == 'b') ? 2 : 1;
-    }
-    return cached;
-}
-
-// MB200_ROWS_OVERLAP: 0 = plain launches; 1 (default) = programmatic dependent launch, the kernel waits for the previous
-// grid's completion before its first input load (always correct); 2 = no wait: consecutive updates overlap drain and
-// ramp-up — only valid when the inputs were complete before the PREVIOUS kernel of the stream started (e.g. a replay of
-// resident batches), because a foreign producer that triggers its dependents early would otherwise race with the loads.
-static int rows_overlap_mode() {
-    static int cached = -1;
-    if (cached < 0) {
-        const char* e = getenv("MB200_ROWS_OVERLAP");
-        cached = (e && e[0] >= '0' && e[0] <= '2') ? (e[0] - '0') : 1;
-    }
-    return cached;
-}
-static bool rows_overlap_enabled() { return rows_overlap_mode() != 0; }
-
 // Launch with cudaLaunchAttributeProgrammaticStreamSerialization: the grid may begin while the previous kernel of the
 // stream is still draining (that kernel opts in with griddepcontrol.launch_dependents).  Only used for launches whose
 // sole shared data are commutative atomics on the state.
@@ -384,57 +240,24 @@ static int resident_blocks(Kernel k, int threads, size_t smem) {
     return blocks;
 }
 
-template <typename T, typename Sink, bool kI64, int kRows>
-static int launch_bulk(const RowArgs& a, Sink sink, cudaStream_t st, bool& launched) {
-    const size_t stage_bytes = (size_t)a.C * sizeof(T) * kRows;
-    int stages = (int)((200 * 1024) / stage_bytes);
-    if (stages > kBulkMaxStages) stages = kBulkMaxStages;
-    launched = false;
-    if (stages < 3 || a.n_outer < 4 * kRows) return 0;
-    auto kern = rows_bulk_kernel<T, Sink, kI64, kRows>;
-    MB200_CUDA_OK(ensure_dynamic_smem(kern, 227 * 1024 - 512));
-    const long long tiles = (a.n_outer + kRows - 1) / kRows;
-    int grid = sm_count();
-    if (tiles < grid) grid = (int)tiles;
-    kern<<<grid, (kRows + 1) * 32, (size_t)stages * stage_bytes, st>>>(a, sink, stages);
-    launched = true;
-    return 0;
-}
-
 template <typename T, typename Sink, bool kI64>
 static int launch_rows(const RowArgs& a, Sink sink, size_t smem, cudaStream_t st) {
     const size_t row_bytes = (size_t)a.C * sizeof(T);
     const bool vec_ok = sizeof(T) <= 4 && a.inner == 1 && a.C >= 32 && (row_bytes % 16 == 0) &&
                         ((reinterpret_cast<uintptr_t>(a.preds) & 15) == 0);
-    if (a.inner == 1 && a.C >= 32) {
-        if (vec_ok) {
-            if constexpr (sizeof(T) <= 4) {
-                const int ov = rows_path_override();
-                bool launched = false;
-                if (smem == 0 && ov == 2) {
-                    if (int rc = launch_bulk<T, Sink, kI64, 16>(a, sink, st, launched)) return rc;
-                }
-                if (!launched) {
-                    auto kern = rows_vec_kernel<T, Sink, kI64>;
-                    const int grid = grid_for(a.n_outer, kRowThreads / 32, resident_blocks(kern, kRowThreads, smem));
-                    if constexpr (Sink::kOverlapSafe) {
-                        if (rows_overlap_enabled()) {
-                            RowArgs ao = a;
-                            ao.pdl_wait = rows_overlap_mode() == 1 || Sink::kMustWait;  // see sinks.cuh
-                            MB200_CUDA_OK(launch_overlapped(kern, grid, kRowThreads, smem, st, ao, sink));
-                        } else {
-                            kern<<<grid, kRowThreads, smem, st>>>(a, sink);
-                        }
-                    } else {
-                        kern<<<grid, kRowThreads, smem, st>>>(a, sink);
-                    }
-                }
-            }
-        } else {
-            auto kern = rows_scalar_kernel<T, Sink, kI64>;
+    if (vec_ok) {
+        if constexpr (sizeof(T) <= 4) {
+            auto kern = rows_vec_kernel<T, Sink, kI64>;
             const int grid = grid_for(a.n_outer, kRowThreads / 32, resident_blocks(kern, kRowThreads, smem));
-            kern<<<grid, kRowThreads, smem, st>>>(a, sink);
+            if constexpr (Sink::kOverlapSafe)
+                MB200_CUDA_OK(launch_overlapped(kern, grid, kRowThreads, smem, st, a, sink));
+            else
+                kern<<<grid, kRowThreads, smem, st>>>(a, sink);
         }
+    } else if (a.inner == 1 && a.C >= 32) {
+        auto kern = rows_scalar_kernel<T, Sink, kI64>;
+        const int grid = grid_for(a.n_outer, kRowThreads / 32, resident_blocks(kern, kRowThreads, smem));
+        kern<<<grid, kRowThreads, smem, st>>>(a, sink);
     } else {
         auto kern = rows_strided_kernel<T, Sink, kI64>;
         const int grid = grid_for(a.n_outer * a.inner, kRowThreads, resident_blocks(kern, kRowThreads, smem));
@@ -542,7 +365,7 @@ extern "C" int mb200_multiclass_stat_scores_update(const void* preds, int preds_
     }
     // Large launches: rows only RED into the workspace, the fold follows as its own one-CTA kernel (see sinks.cuh kDeferFold);
     // small ones keep the single launch (an extra launch costs more host time than the fold tail costs device time).
-    if (preds_has_class_dim && inner == 1 && n_outer * num_classes >= (1ll << 24) && rows_overlap_enabled()) {
+    if (preds_has_class_dim && inner == 1 && n_outer * num_classes >= (1ll << 24)) {
         StatsSink<false, true> s{(long long*)tp, (long long*)fp, (long long*)tn, (long long*)fn, (long long*)workspace,
                                  (int)num_classes, micro};
         if (int rc = dispatch_rows(preds_dtype, preds_has_class_dim, a, s, 0, st)) return rc;

@@ -16,7 +16,6 @@ struct ArgmaxOutSink {
     __device__ __forceinline__ void finish(Local&) {}
     static constexpr bool kNeedsTarget = false;
     static constexpr bool kOverlapSafe = false;
-    static constexpr bool kMustWait = true;
 };
 
 // confmat[t, p] += 1 straight into the (L2-resident) state; optional shared-memory privatisation for tiny C.
@@ -29,7 +28,6 @@ struct ConfmatSink {
     // Two consecutive launches may overlap (programmatic dependent launch): all they share is the state, and they only
     // ever touch it with commutative 64-bit REDs.
     static constexpr bool kOverlapSafe = true;
-    static constexpr bool kMustWait = false;  // the opt-in no-wait overlap (MB200_ROWS_OVERLAP=2) is allowed
     __device__ __forceinline__ void block_init() {
         if (kSmem) {
             extern __shared__ unsigned sh_bins[];
@@ -75,9 +73,9 @@ struct StatsSink {
     };
     static constexpr bool kNeedsTarget = true;
     // self-cleaning workspace + last-CTA ticket: launches must not overlap — unless the fold is deferred: then this grid only
-    // issues commutative REDs, and its successor in the stream (the fold kernel) waits for it explicitly
+    // issues commutative REDs, and its successor in the stream (the fold kernel) waits for it explicitly.  Its own
+    // griddepcontrol.wait also orders its REDs after the previous update's fold, which re-zeroes this workspace.
     static constexpr bool kOverlapSafe = kDeferFold;
-    static constexpr bool kMustWait = true;  // the previous update's fold kernel zeroes the workspace these REDs go to
     __device__ __forceinline__ void block_init() {
         if (kSmem) {
             extern __shared__ unsigned sh_bins[];
@@ -214,7 +212,6 @@ struct SamplewiseSink {
     struct Local {};
     static constexpr bool kNeedsTarget = true;
     static constexpr bool kOverlapSafe = false;
-    static constexpr bool kMustWait = true;
     __device__ __forceinline__ void block_init() {}
     __device__ __forceinline__ void init(Local&) {}
     __device__ __forceinline__ void row(Local&, long long idx, long long t, int p) {

@@ -2,8 +2,9 @@
 `..._samplewise`, `mb200_argmax_rows`; csrc/confmat.cu) against the reference's own chain of torch ops
 (oracle/multiclass_counts.py) run on the same GPU, bit for bit, on every launch path and sink of `confmat.cu`:
 
-  kernels  vec (warp per row, 16-byte loads, programmatic dependent launch), bulk (`cp.async.bulk` ring, opt-in), scalar
-           (float64, odd row bytes, misaligned base), strided (C < 32, `[N, C, d...]`), labels (integer predictions), top-k
+  kernels  vec (warp per row, 16-byte loads, programmatic dependent launch for the confusion-matrix and deferred sinks),
+           scalar (float64, odd row bytes, misaligned base), strided (C < 32, `[N, C, d...]`), labels (integer
+           predictions), top-k
   sinks    confusion matrix in shared memory / global; stat scores in shared memory / global / deferred fold, micro and
            macro; samplewise; argmax
 
@@ -20,10 +21,6 @@ a subnormal maximum among zeros and all-equal rows; and every float16 / bfloat16
 `ignore_index` is compared as the reference compares it: ATen casts the Python int to the target's dtype, so with uint8
 targets 257 drops class 1 and -1 drops 255.
 """
-import os
-import subprocess
-import sys
-
 import pytest
 import torch
 
@@ -37,21 +34,11 @@ FLOATS = [torch.float32, torch.float16, torch.bfloat16]
 SIZES = [1, 2, 31, 32, 33, 63, 64, 65, 255, 256, 257, 511, 512, 513, 520, 1000, 1023, 1024, 1025, 1032, 2047, 2048, 2049,
          4100]
 LABEL_DTYPES = [torch.int8, torch.uint8, torch.int16, torch.int32, torch.int64]
-ENV_VARS = ("MB200_ROWS_OVERLAP", "MB200_ROWS_PATH")
 
 
 # ------------------------------------------------------------------------------------------------------------------
 # the dispatch of confmat.cu, restated
 # ------------------------------------------------------------------------------------------------------------------
-def overlap_mode() -> int:
-    e = os.environ.get("MB200_ROWS_OVERLAP", "")
-    return int(e[0]) if e[:1] in ("0", "1", "2") else 1
-
-
-def bulk_requested() -> bool:
-    return os.environ.get("MB200_ROWS_PATH", "")[:1] == "b"
-
-
 def geometry(preds, target):
     if preds.ndim == target.ndim + 1:
         inner = 1
@@ -62,7 +49,8 @@ def geometry(preds, target):
 
 
 def path_of(entry, preds, target, num_classes, micro=False):
-    """(kernel, sink) that `entry` launches: kernel in vec / vec_nowait / vec_plain / bulk / scalar / strided / labels / topk."""
+    """(kernel, sink) that `entry` launches: kernel in vec (programmatic launch) / vec_plain / scalar / strided / labels /
+    topk."""
     C = num_classes
     class_dim, n_outer, inner = geometry(preds, target)
     total = n_outer * inner
@@ -71,7 +59,7 @@ def path_of(entry, preds, target, num_classes, micro=False):
     elif entry == "stats":
         if not micro and C <= 256 and total >= 4096 and total >= 16 * C:
             sink = "stats_smem"
-        elif class_dim and inner == 1 and n_outer * C >= 1 << 24 and overlap_mode() != 0:
+        elif class_dim and inner == 1 and n_outer * C >= 1 << 24:
             sink = "stats_deferred"
         else:
             sink = "stats_global"
@@ -86,14 +74,8 @@ def path_of(entry, preds, target, num_classes, micro=False):
     item = preds.element_size()
     if not (item <= 4 and (C * item) % 16 == 0 and preds.data_ptr() % 16 == 0):
         return "scalar", sink
-    smem = sink in ("confmat_smem", "stats_smem")
-    if bulk_requested() and not smem:
-        stages = min(8, (200 * 1024) // (C * item * 16))
-        if stages >= 3 and n_outer >= 64:
-            return "bulk", sink
-    if sink in ("confmat_smem", "confmat_global", "stats_deferred") and overlap_mode() != 0:
-        must_wait = sink == "stats_deferred"
-        return ("vec" if overlap_mode() == 1 or must_wait else "vec_nowait"), sink
+    if sink in ("confmat_smem", "confmat_global", "stats_deferred"):
+        return "vec", sink
     return "vec_plain", sink
 
 
@@ -273,10 +255,6 @@ def check_argmax(preds):
     return path
 
 
-def vec_kernel() -> str:
-    return {0: "vec_plain", 1: "vec", 2: "vec_nowait"}[overlap_mode()]
-
-
 # ------------------------------------------------------------------------------------------------------------------
 # launch paths x sizes
 # ------------------------------------------------------------------------------------------------------------------
@@ -301,7 +279,7 @@ def test_row_paths_and_sizes(C, dtype):
         for ign in (None, -1, 0, C - 1, C):
             t = targets(n, C, torch.int64, ign, seed=C + n)
             cm_sink = "confmat_smem" if C * C <= 4096 and n >= 4096 else "confmat_global"
-            check_confmat(x, t, C, ign, (vec_kernel() if base == "vec" else base, cm_sink))
+            check_confmat(x, t, C, ign, (base, cm_sink))
             st_sink = "stats_smem" if C <= 256 and n >= 4096 else "stats_global"
             check_stats(x, t, C, ign, False, ("vec_plain" if base == "vec" else base, st_sink))
         t = targets(n, C, torch.int64, -1, seed=C)
@@ -386,8 +364,7 @@ def test_target_dtypes_on_the_float_paths(tdtype):
                 if ign == -1 and not tdtype.is_signed:
                     continue
                 t = targets(n, c, tdtype, ign, seed=17).reshape(tshape)
-                k = label if label != "vec" else vec_kernel()
-                check_confmat(x, t, c, ign, (k, "confmat_global"))
+                check_confmat(x, t, c, ign, (label, "confmat_global"))
                 check_stats(x, t, c, ign, False, (label if label != "vec" else "vec_plain", "stats_smem"))
                 check_stats(x, t, c, ign, True, (label if label != "vec" else "vec_plain", "stats_global"))
             if label != "strided":
@@ -409,7 +386,7 @@ def test_ignore_index_is_compared_in_the_target_dtype(tdtype, ign):
             t[::5] = w
             assert bool((t == ign).any()) and int((t == ign).sum()) == int((t == w).sum())
             k = row_kernel(xx)
-            check_confmat(xx, t, c, ign, (vec_kernel() if k == "vec" else k, "confmat_global" if c * c > 4096 else "confmat_smem"))
+            check_confmat(xx, t, c, ign, (k, "confmat_global" if c * c > 4096 else "confmat_smem"))
             check_stats(xx, t, c, ign, False, ("vec_plain" if k == "vec" else k, "stats_smem"))
             check_stats(xx, t, c, ign, True, ("vec_plain" if k == "vec" else k, "stats_global"))
             check_topk(xx, t, c, 2, ign)
@@ -463,7 +440,7 @@ def test_every_half_precision_pattern_as_a_row_maximum(dtype):
     x = every_pattern_rows(dtype, C)
     t = targets(65536, C, torch.int64, -1, seed=26)
     assert check_argmax(x) == ("vec_plain", "argmax")
-    check_confmat(x, t, C, -1, (vec_kernel(), "confmat_global"))
+    check_confmat(x, t, C, -1, ("vec", "confmat_global"))
     check_stats(x, t, C, -1, False, ("vec", "stats_deferred"))
     check_stats(x[:4096], t[:4096], C, -1, False, ("vec_plain", "stats_global"))
     xs = misaligned(x)
@@ -489,8 +466,7 @@ def test_error_word_on_out_of_range_targets(where):
         for tdt, ign in ((torch.int64, None), (torch.int64, -1), (torch.int64, C), (torch.uint8, 257), (torch.int8, 255)):
             t = targets(n, C, tdt, ign, seed=30, bad=(r,))
             k = row_kernel(x)
-            check_confmat(x, t, C, ign, (vec_kernel() if k == "vec" else k,
-                                         "confmat_smem" if C * C <= 4096 and n >= 4096 else "confmat_global"))
+            check_confmat(x, t, C, ign, (k, "confmat_smem" if C * C <= 4096 and n >= 4096 else "confmat_global"))
             check_stats(x, t, C, ign, False, ("vec_plain" if k == "vec" else k, "stats_smem"))
             check_stats(x, t, C, ign, True, ("vec_plain" if k == "vec" else k, "stats_global"))
             if k != "strided":
@@ -554,7 +530,7 @@ def test_more_than_2_31_scores():
     assert x.numel() > 2**31
     cm = torch.zeros(C, C, dtype=torch.int64, device=DEV)
     states, ws = stats_state(C, False)
-    assert path_of("confmat", x, t, C) == (vec_kernel(), "confmat_global")
+    assert path_of("confmat", x, t, C) == ("vec", "confmat_global")
     assert path_of("stats", x, t, C) == ("vec", "stats_deferred")
     _native.multiclass_confmat_update_(cm, x, t, C, -1)
     _native.multiclass_stat_scores_update_(*states, ws, x, t, C, -1, False)
@@ -570,11 +546,11 @@ def test_more_than_2_31_scores():
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# the environment-selected paths (read once per process by confmat.cu: one child process per setting)
+# back-to-back updates: consecutive programmatic launches into one state
 # ------------------------------------------------------------------------------------------------------------------
-def test_reduced_matrix():
-    """The matrix the environment-selected paths run (in this process: the default, PDL with wait): each sink on the vec
-    path at C = 32 / 1000 / 1024 in every score dtype, and eight distinct resident batches updated back to back."""
+def test_back_to_back_updates():
+    """Each sink on the vec path at C = 32 / 1000 / 1024 in every score dtype, then eight distinct resident batches updated
+    back to back with no host synchronisation in between: each launch waits for the previous grid of the stream."""
     for dtype in FLOATS:
         for C, n in ((32, 4096), (1000, 4096), (1024, 1200)):
             x = rows(n, C, dtype, seed=41)
@@ -592,9 +568,8 @@ def test_reduced_matrix():
     ts = [targets(n, C, torch.int64, -1, seed=60 + i) for i in range(8)]
     cm_path = path_of("confmat", xs[0], ts[0], C)
     st_path = path_of("stats", xs[0], ts[0], C)
-    assert cm_path == ("bulk" if bulk_requested() else vec_kernel(), "confmat_global")
-    assert st_path == ("bulk" if bulk_requested() else "vec_plain" if overlap_mode() == 0 else "vec",
-                       "stats_global" if overlap_mode() == 0 else "stats_deferred")
+    assert cm_path == ("vec", "confmat_global")
+    assert st_path == ("vec", "stats_deferred")
     cm = torch.zeros(C, C, dtype=torch.int64, device=DEV)
     states, ws = stats_state(C, False)
     for x, t in zip(xs, ts):  # back to back, no host synchronisation in between
@@ -609,21 +584,6 @@ def test_reduced_matrix():
     for x, t in zip(xs, ts):
         _native.multiclass_confmat_update_(cm, x, t, C, -1)
     assert torch.equal(cm, want_cm), "confusion matrix alone, back to back"
-
-
-@pytest.mark.parametrize("setting", ["MB200_ROWS_OVERLAP=0", "MB200_ROWS_OVERLAP=2", "MB200_ROWS_PATH=bulk"])
-def test_env_selected_paths(setting):
-    name, value = setting.split("=")
-    env = {k: v for k, v in os.environ.items() if k not in ENV_VARS}
-    env[name] = value
-    env["PYTHONDONTWRITEBYTECODE"] = "1"
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    flags = ["-s"] if sys.flags.no_user_site else []
-    proc = subprocess.run(
-        [sys.executable, *flags, "-m", "pytest", "-q", "-x", "-p", "no:cacheprovider",
-         f"{os.path.abspath(__file__)}::test_reduced_matrix"],
-        cwd=root, env=env, capture_output=True, text=True, timeout=900)
-    assert proc.returncode == 0 and " passed" in proc.stdout, proc.stdout[-3000:] + proc.stderr[-2000:]
 
 
 # ------------------------------------------------------------------------------------------------------------------
