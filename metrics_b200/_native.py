@@ -151,11 +151,17 @@ SIGNATURES = {
     "mb200_spearman_corrcoef": ("i", "pipiqqpidpqpp"),
     "mb200_kendall_rank_corrcoef": ("i", "pipiqqiipippqpp"),
 }
+# include/mb200_panoptic.h (K18), kept outside the include/metrics_b200*.h set that tests/test_abi.py sweeps wrapper by
+# wrapper; tests/test_panoptic_abi.py holds it to the same checks
+PANOPTIC_SIGNATURES = {
+    "mb200_panoptic_scratch_bytes": ("q", "qqqqqqii"),
+    "mb200_panoptic_update": ("i", "pipiqqpqqiiqqqpppppqpp"),
+}
 
 
 def declare_signatures(handle) -> None:
     """Set ``restype`` / ``argtypes`` of every exported function on a loaded library handle."""
-    for name, (ret, args) in SIGNATURES.items():
+    for name, (ret, args) in {**SIGNATURES, **PANOPTIC_SIGNATURES}.items():
         fn = getattr(handle, name)
         fn.restype = _C_TYPES[ret]
         fn.argtypes = [_C_TYPES[a] for a in args]
@@ -1268,3 +1274,79 @@ def kendall_rank_corrcoef(preds: Tensor, target: Tensor, variant: str, alternati
         tau = tau.reshape(())
         p_value = None if p_value is None else p_value.reshape(())
     return tau, p_value
+
+
+# ----------------------------------------------------------------------------------------------------------
+# K18 wrapper (panoptic quality, include/metrics_b200_panoptic.h)
+# ----------------------------------------------------------------------------------------------------------
+PQ_UNKNOWN_PREDS, FLAG_CAPACITY = 1, 8
+# per-image hash-table slots of the first pass: an image with up to 1024 distinct pred or target colors and 4096 color pairs
+# fits; a larger one sets FLAG_CAPACITY and the update is repeated with tables that cannot fill
+PANOPTIC_COLOR_CAPACITY, PANOPTIC_PAIR_CAPACITY = 2048, 8192
+PANOPTIC_RERUN_BYTES = 1 << 30  # hash tables of one launch of that repeat, at least one image
+PANOPTIC_MAX_PIXELS = 1 << 30
+
+
+def _pow2_at_least(v: int) -> int:
+    return 1 << max(6, (int(v) - 1).bit_length())
+
+
+def panoptic_categories(things, stuffs, device) -> Tensor:
+    """The ``categories`` argument of K18: the category ids in ascending order, then the continuous id of each (things in
+    ascending id order first, then stuffs), int64 on ``device``."""
+    cid = {c: i for i, c in enumerate(sorted(things))}
+    cid.update({c: len(things) + i for i, c in enumerate(sorted(stuffs))})
+    ids = sorted(cid)
+    return torch.tensor(ids + [cid[c] for c in ids], dtype=torch.int64, device=device)
+
+
+def _pair_rows(x: Tensor) -> Tensor:
+    """``[n, ..., 2]`` as a contiguous tensor whose start is aligned to one (category, instance) pair."""
+    x = x.contiguous()
+    if x.data_ptr() % (2 * x.element_size()):
+        x = x.clone()
+    return x
+
+
+def panoptic_update_(iou_sum: Tensor, true_positives: Tensor, false_positives: Tensor, false_negatives: Tensor, preds: Tensor,
+                     target: Tensor, categories: Tensor, num_things: int, modified: bool, allow_unknown_preds: bool) -> bool:
+    """K18 (``mb200_panoptic_update``): add one batch of ``[n, *spatial, 2]`` integer panoptic maps to the four ``[K]``
+    states in place.  Returns True, with the states unchanged, when ``preds`` holds a category that is neither a thing nor
+    a stuff and ``allow_unknown_preds`` is False.  One host synchronisation: the error word; an image with more distinct
+    segments than the first pass's tables is counted again with tables sized for one segment per pixel."""
+    dev = require_cuda(preds, target, iou_sum)
+    n = preds.shape[0]
+    pixels = 1
+    for s in preds.shape[1:-1]:
+        pixels *= s
+    if pixels > PANOPTIC_MAX_PIXELS:
+        raise ValueError(f"metrics_b200: panoptic quality supports at most 2^30 points per image, got {pixels}.")
+    preds, target = _pair_rows(preds), _pair_rows(target)
+    k = categories.numel() // 2
+    err = torch.empty(1, dtype=torch.int32, device=dev)
+    lib_ = lib()
+
+    def run(per_launch: int, color_capacity: int, pair_capacity: int) -> None:
+        nbytes = int(lib_.mb200_panoptic_scratch_bytes(n, pixels, k, per_launch, color_capacity, pair_capacity, tag(preds),
+                                                       tag(target)))
+        if nbytes < 0:
+            raise ValueError(f"metrics_b200: unsupported panoptic inputs ({preds.dtype}, {target.dtype}, {k} categories)")
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        with on_device(dev):
+            rc = lib_.mb200_panoptic_update(preds.data_ptr(), tag(preds), target.data_ptr(), tag(target), n, pixels,
+                                            categories.data_ptr(), k, int(num_things), int(bool(modified)),
+                                            int(bool(allow_unknown_preds)), per_launch, color_capacity, pair_capacity,
+                                            iou_sum.data_ptr(), true_positives.data_ptr(), false_positives.data_ptr(),
+                                            false_negatives.data_ptr(), scratch.data_ptr(), nbytes, err.data_ptr(),
+                                            stream_handle(dev))
+        check(rc, "panoptic_update")
+
+    worst = _pow2_at_least(2 * max(pixels, 1))
+    run(max(n, 1), min(PANOPTIC_COLOR_CAPACITY, worst), min(PANOPTIC_PAIR_CAPACITY, worst))
+    flags = int(err.item())
+    if flags & PQ_UNKNOWN_PREDS:
+        return True
+    if flags & FLAG_CAPACITY:
+        per_image = int(lib_.mb200_panoptic_scratch_bytes(1, pixels, k, 1, worst, worst, tag(preds), tag(target)))
+        run(max(1, min(n, PANOPTIC_RERUN_BYTES // per_image)), worst, worst)
+    return False

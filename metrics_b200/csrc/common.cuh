@@ -71,6 +71,20 @@ int with_float_type(int dtype, F&& f) {
     }
 }
 
+// Returns f(As<T>{}) for the integer type T of `dtype`: long long, int, short, signed char, unsigned char.  MB200_BOOL and
+// every non-integer tag return kNoType without calling f.
+template <typename F>
+int with_label_type(int dtype, F&& f) {
+    switch (dtype) {
+        case MB200_I64: return f(As<long long>{});
+        case MB200_I32: return f(As<int>{});
+        case MB200_I16: return f(As<short>{});
+        case MB200_I8: return f(As<signed char>{});
+        case MB200_U8: return f(As<unsigned char>{});
+        default: return kNoType;
+    }
+}
+
 // ---- device helpers -------------------------------------------------------------------------------
 // Streaming 16-byte load: data is consumed exactly once, keep it out of L1.
 __device__ __forceinline__ uint4 ld_stream16(const void* p) {
