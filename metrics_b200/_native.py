@@ -157,11 +157,16 @@ PANOPTIC_SIGNATURES = {
     "mb200_panoptic_scratch_bytes": ("q", "qqqqqqii"),
     "mb200_panoptic_update": ("i", "pipiqqpqqiiqqqpppppqpp"),
 }
+# include/mb200_hausdorff.h (K19), outside that set for the same reason; tests/test_hausdorff_abi.py checks it
+HAUSDORFF_SIGNATURES = {
+    "mb200_hausdorff_scratch_bytes": ("q", "qqiq"),
+    "mb200_hausdorff_distance": ("i", "pipiiqqqqqqqqqqqqiiiddiqppqpp"),
+}
 
 
 def declare_signatures(handle) -> None:
     """Set ``restype`` / ``argtypes`` of every exported function on a loaded library handle."""
-    for name, (ret, args) in {**SIGNATURES, **PANOPTIC_SIGNATURES}.items():
+    for name, (ret, args) in {**SIGNATURES, **PANOPTIC_SIGNATURES, **HAUSDORFF_SIGNATURES}.items():
         fn = getattr(handle, name)
         fn.restype = _C_TYPES[ret]
         fn.argtypes = [_C_TYPES[a] for a in args]
@@ -1350,3 +1355,50 @@ def panoptic_update_(iou_sum: Tensor, true_positives: Tensor, false_positives: T
         per_image = int(lib_.mb200_panoptic_scratch_bytes(1, pixels, k, 1, worst, worst, tag(preds), tag(target)))
         run(max(1, min(n, PANOPTIC_RERUN_BYTES // per_image)), worst, worst)
     return False
+
+
+# ----------------------------------------------------------------------------------------------------------
+# K19 wrapper (Hausdorff distance, include/mb200_hausdorff.h)
+# ----------------------------------------------------------------------------------------------------------
+HD_PREDS_NOT_BINARY, HD_TARGET_NOT_BINARY, HD_NO_EDGES = 0, 1, 2
+HD_METRICS = {"euclidean": 0, "chessboard": 1, "taxicab": 2}
+# scratch of one launch: pairs are processed as many at a time as fit, at least one
+HAUSDORFF_SCRATCH_BYTES = 1 << 28
+
+
+def hausdorff_distance(preds: Tensor, target: Tensor, num_classes: int, index_format: bool, drop_background: bool,
+                       distance_metric: str, spacing: tuple, directed: bool) -> tuple[Tensor, Tensor]:
+    """K19 (``mb200_hausdorff_distance``): the ``[N, C']`` float32 Hausdorff distances of 2-D masks and the int64 ``[2]``
+    error word, read in place through their strides.  Index format: int64 labels ``[N, H, W]``, ``C = num_classes``.
+    One-hot format: ``[N, C, H, W]`` integer or bool tensors, ``C = preds.shape[1]``.  ``spacing``: two Python ints or
+    floats; an int is int64 arithmetic, a float float32.  ``err[0]``: ``4 * pair + HD_*`` of the first failing pair, or
+    -1; ``err[1]``: ``SEG_*`` label bits.  No host synchronisation."""
+    dev = require_cuda(preds, target)
+    n, h, w = preds.shape[0], preds.shape[-2], preds.shape[-1]
+    c = int(num_classes) if index_format else preds.shape[1]
+    cp = c - 1 if drop_background and c > 1 else c
+    out = torch.empty((n, cp), dtype=torch.float32, device=dev)
+    err = torch.empty(2, dtype=torch.int64, device=dev)
+    if index_format:
+        ps = (preds.stride(0), 0, preds.stride(1), preds.stride(2))
+        ts = (target.stride(0), 0, target.stride(1), target.stride(2))
+    else:
+        ps, ts = preds.stride(), target.stride()
+    int_mask = sum(1 << k for k, v in enumerate(spacing) if isinstance(v, int))
+    lib_ = lib()
+    per_pair = int(lib_.mb200_hausdorff_scratch_bytes(max(h, 1), max(w, 1), int(bool(directed)), 1))
+    per_launch = max(1, min(n * cp, HAUSDORFF_SCRATCH_BYTES // max(per_pair, 1)))
+    nbytes = int(lib_.mb200_hausdorff_scratch_bytes(max(h, 1), max(w, 1), int(bool(directed)), per_launch))
+    if per_pair < 0 or nbytes < 0:
+        raise ValueError(f"metrics_b200: unsupported image size {h} x {w}")
+    scratch = torch.empty(nbytes if n * cp else 0, dtype=torch.uint8, device=dev)
+    with on_device(dev):
+        rc = lib_.mb200_hausdorff_distance(
+            preds.data_ptr(), tag(preds), target.data_ptr(), tag(target), 0 if index_format else 1, n, c, h, w, *ps, *ts,
+            int(bool(drop_background)), HD_METRICS[distance_metric], int_mask, float(spacing[0]), float(spacing[1]),
+            int(bool(directed)), per_launch, out.data_ptr(), scratch.data_ptr(), scratch.numel(), err.data_ptr(),
+            stream_handle(dev),
+        )
+    if rc:
+        check(rc, "hausdorff_distance")
+    return out, err
