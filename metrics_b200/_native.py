@@ -44,6 +44,7 @@ def _ops():
 FLAG_TARGET_RANGE = 1
 FLAG_PREDS_RANGE = 2
 FLAG_SPIN_TIMEOUT = 4
+FLAG_CAPACITY = 8
 
 
 class NativeLibraryError(RuntimeError):
@@ -150,15 +151,10 @@ SIGNATURES = {
     "mb200_rankcorr_scratch_bytes": ("q", "qqi"),
     "mb200_spearman_corrcoef": ("i", "pipiqqpidpqpp"),
     "mb200_kendall_rank_corrcoef": ("i", "pipiqqiipippqpp"),
-}
-# include/mb200_panoptic.h (K18), kept outside the include/metrics_b200*.h set that tests/test_abi.py sweeps wrapper by
-# wrapper; tests/test_panoptic_abi.py holds it to the same checks
-PANOPTIC_SIGNATURES = {
+    # include/metrics_b200_panoptic.h
     "mb200_panoptic_scratch_bytes": ("q", "qqqqqqii"),
     "mb200_panoptic_update": ("i", "pipiqqpqqiiqqqpppppqpp"),
-}
-# include/mb200_hausdorff.h (K19), outside that set for the same reason; tests/test_hausdorff_abi.py checks it
-HAUSDORFF_SIGNATURES = {
+    # include/metrics_b200_hausdorff.h
     "mb200_hausdorff_scratch_bytes": ("q", "qqiq"),
     "mb200_hausdorff_distance": ("i", "pipiiqqqqqqqqqqqqiiiddiqppqpp"),
 }
@@ -166,7 +162,7 @@ HAUSDORFF_SIGNATURES = {
 
 def declare_signatures(handle) -> None:
     """Set ``restype`` / ``argtypes`` of every exported function on a loaded library handle."""
-    for name, (ret, args) in {**SIGNATURES, **PANOPTIC_SIGNATURES, **HAUSDORFF_SIGNATURES}.items():
+    for name, (ret, args) in SIGNATURES.items():
         fn = getattr(handle, name)
         fn.restype = _C_TYPES[ret]
         fn.argtypes = [_C_TYPES[a] for a in args]
@@ -1284,7 +1280,7 @@ def kendall_rank_corrcoef(preds: Tensor, target: Tensor, variant: str, alternati
 # ----------------------------------------------------------------------------------------------------------
 # K18 wrapper (panoptic quality, include/metrics_b200_panoptic.h)
 # ----------------------------------------------------------------------------------------------------------
-PQ_UNKNOWN_PREDS, FLAG_CAPACITY = 1, 8
+PQ_UNKNOWN_PREDS = 1  # with FLAG_CAPACITY, the bits of K18's error word
 # per-image hash-table slots of the first pass: an image with up to 1024 distinct pred or target colors and 4096 color pairs
 # fits; a larger one sets FLAG_CAPACITY and the update is repeated with tables that cannot fill
 PANOPTIC_COLOR_CAPACITY, PANOPTIC_PAIR_CAPACITY = 2048, 8192
@@ -1358,7 +1354,7 @@ def panoptic_update_(iou_sum: Tensor, true_positives: Tensor, false_positives: T
 
 
 # ----------------------------------------------------------------------------------------------------------
-# K19 wrapper (Hausdorff distance, include/mb200_hausdorff.h)
+# K19 wrapper (Hausdorff distance, include/metrics_b200_hausdorff.h)
 # ----------------------------------------------------------------------------------------------------------
 HD_PREDS_NOT_BINARY, HD_TARGET_NOT_BINARY, HD_NO_EDGES = 0, 1, 2
 HD_METRICS = {"euclidean": 0, "chessboard": 1, "taxicab": 2}

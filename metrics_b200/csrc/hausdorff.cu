@@ -25,7 +25,7 @@
 #include <algorithm>
 
 #include "common.cuh"
-#include "../../include/mb200_hausdorff.h"
+#include "../../include/metrics_b200_hausdorff.h"
 
 namespace mb200 {
 

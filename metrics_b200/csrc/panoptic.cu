@@ -32,7 +32,7 @@
 #include <algorithm>
 
 #include "common.cuh"
-#include "../../include/mb200_panoptic.h"
+#include "../../include/metrics_b200_panoptic.h"
 
 namespace mb200 {
 

@@ -1,4 +1,5 @@
-"""CPU and GPU: every C entry point that takes a score dtype tag, called directly through `_native.lib()`.
+"""CPU and GPU: every C entry point that takes a score dtype tag, called directly through `_native.lib()`; for K16's group
+sort that is its graded target, for K18 and K19 their label maps.  Where an entry point takes two tags, one is held fixed.
 
 A tag the entry point does not accept must come back with its own error code and message before any CUDA work: no launch is
 counted and, on a box without a GPU, no CUDA error masks the dtype error.  On such a box every accepted tag must get past the
@@ -13,7 +14,7 @@ F32, F16, BF16, F64, I64 = _native.F32, _native.F16, _native.BF16, _native.F64, 
 FLOAT = {F32, F16, BF16, F64}
 FLOAT_NO_F64 = {F32, F16, BF16}
 LABELS = {_native.I64, _native.I32, _native.I16, _native.I8, _native.U8, _native.BOOL}
-TAGS = list(range(10)) + [10]  # every mb200_dtype and one past the end
+TAGS = [-1] + list(range(10)) + [10]  # every mb200_dtype and one past either end
 
 INVALID, UNSUPPORTED = -1, -3
 N, C = 16, 3
@@ -43,6 +44,14 @@ REGRESSION_MSG = "regression inputs must be floating point (dtype tag %d)"
 
 def _curve(fn, b, d):
     return fn(b.p, d, b.t, I64, N, 1, 1, b.ws, NBYTES, b.auroc, b.ap, b.counts, None, None, None, b.err, 0)
+
+
+def _hausdorff(L, b, d, input_format):
+    """Two 4 x 4 images of C classes, int64 target, read through their strides (the class stride is ignored for index labels),
+    every pair in one launch."""
+    s = (C * 16, 16, 4, 1)
+    return L.mb200_hausdorff_distance(b.p, d, b.t, I64, input_format, 2, C, 4, 4, *s, *s, 0, 0, 0, 1.0, 1.0, 0, 2 * C, b.out, b.ws,
+                                      NBYTES, b.err, 0)
 
 
 # name -> (accepted tags, error code, error message format, call(lib, buffers, tag) -> return code)
@@ -103,6 +112,23 @@ ENTRIES = {
     "segmentation_one_hot": (FLOAT_NO_F64 | LABELS, INVALID, "unsupported dtype tag %d",
                              lambda L, b, d: L.mb200_segmentation_overlap_counts(
                                  b.p, d, b.t, d, 2, C, N, 1, 0, C * N, C * N, 1, 0, b.out, b.ws, NBYTES, b.err, 0)),
+    # the target's tag is the one varied
+    "retrieval_sort": ({I64, F32}, INVALID, "target must be int64 or float32 (dtype tag %d)", lambda L, b, d: L.mb200_retrieval_sort(
+        b.idx, b.p, b.t, d, N, 0, 0, b.sort_keys, b.out, b.offsets, b.info, b.ws, NBYTES, 0)),
+    # the other tags float32
+    "spearman": (FLOAT, INVALID, "spearman inputs and output must be floating point (dtype tags %d, 0, 0)",
+                 lambda L, b, d: L.mb200_spearman_corrcoef(b.p, d, b.t, F32, N, 1, b.out, F32, 1e-6, b.ws, NBYTES, b.err, 0)),
+    "kendall": (FLOAT | {_native.I32, I64}, INVALID, "kendall inputs must be floating point, int32 or int64 (dtype tags %d, 0)",
+                lambda L, b, d: L.mb200_kendall_rank_corrcoef(b.p, d, b.t, F32, N, 1, 1, 0, b.out, F32, None, b.ws, NBYTES, b.err, 0)),
+    "kendall_target": (FLOAT | {_native.I32, I64}, INVALID, "kendall inputs must be floating point, int32 or int64 (dtype tags 0, %d)",
+                       lambda L, b, d: L.mb200_kendall_rank_corrcoef(b.p, F32, b.t, d, N, 1, 1, 0, b.out, F32, None, b.ws, NBYTES,
+                                                                     b.err, 0)),
+    # int64 target: two images of 8 points, 2 categories, the smallest tables
+    "panoptic_update": (LABELS - {_native.BOOL}, INVALID, "bad sizes, capacities or dtype tags (%d, 4)",
+                        lambda L, b, d: L.mb200_panoptic_update(b.p, d, b.t, I64, 2, 8, b.cats, 2, 1, 0, 0, 2, 64, 64, b.iou, b.tp,
+                                                                b.fp, b.fn, b.ws, NBYTES, b.err, 0)),
+    "hausdorff_one_hot": (LABELS, INVALID, "unsupported dtype tags %d, 4", lambda L, b, d: _hausdorff(L, b, d, 1)),
+    "hausdorff_index": ({I64}, INVALID, "index labels must be int64 (dtype tags %d, 4)", lambda L, b, d: _hausdorff(L, b, d, 0)),
 }
 
 

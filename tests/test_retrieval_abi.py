@@ -1,5 +1,6 @@
-"""CPU: the retrieval C-ABI (include/metrics_b200_retrieval.h): the size guard; tag rejection before any launch; CPU tensors
-rejected.  Its signatures and constants are checked in tests/test_abi.py."""
+"""CPU: the retrieval C-ABI (include/metrics_b200_retrieval.h): the size guard; metric-kind rejection before any launch; CPU
+tensors rejected.  Its signatures and constants are checked in tests/test_abi.py, its dtype tags in
+tests/test_dtype_dispatch_abi.py."""
 import pytest
 import torch
 
@@ -19,16 +20,10 @@ def test_size_guard_is_the_scratch_query():
 
 
 def test_rejected_target_tag_fails_before_any_launch():
+    """The group sort's target tags are checked in tests/test_dtype_dispatch_abi.py; here the metric kind of the evaluation."""
     from metrics_b200 import _native
 
     lib = _native.lib()
-    for tag in range(-1, 11):
-        if tag in (_native.I64, _native.F32):
-            continue
-        before = lib.mb200_launch_count()
-        rc = lib.mb200_retrieval_sort(8, 8, 8, tag, 4, 0, 0, 8, 8, 8, 8, 8, 1 << 20, None)
-        assert rc == -1 and lib.mb200_launch_count() == before, tag
-        assert lib.mb200_last_error().decode() == f"target must be int64 or float32 (dtype tag {tag})"
     before = lib.mb200_launch_count()
     assert lib.mb200_retrieval_evaluate(8, 8, None, 8, 8, 4, 9, 0, 0, 8, 8, 8, 1 << 20, None) == -1
     assert lib.mb200_retrieval_evaluate(8, 8, None, 8, 8, 4, _native.RET_NDCG, 0, 0, 8, 8, 8, 1 << 20, None) == -1
