@@ -350,20 +350,29 @@ MB200_API int mb200_regression_sums(const void* preds, const void* target, int d
  * the multi-threshold confusion matrix confmat[i, (c,) target, score >= thr[i]].
  *  preds      : [n] (num_classes == 1) or [n, num_classes] row-major scores, already sigmoid/softmax-normalised
  *  target     : [n] integer labels; binary: 1 = positive, 0 = negative, anything else skipped
- *  thresholds_sorted : float32 [num_thresholds], ASCENDING (device)
+ *  thresholds_sorted : [num_thresholds] of dtype `thresholds_dtype` (any float or integer tag but bool), ASCENDING (device)
+ *  compare_dtype : the float dtype tag D in which `score >= threshold` is evaluated: the score dtype, F32 or F64 (the
+ *                  score dtype when that is F64).  mb200_binned_curve_compare_dtype gives the reference's choice.
  *  confmat    : int64 [num_thresholds, num_classes, 2, 2] (binary callers view it as [T, 2, 2]), updated in place
  *  scratch    : uint64 [mb200_binned_curve_scratch_words(...)], zero on entry, left zeroed (self-cleaning)
  * ------------------------------------------------------------------------------------------------ */
 MB200_API int64_t mb200_binned_curve_scratch_words(int64_t num_classes, int64_t num_thresholds);
+/* The dtype tag in which the reference compares one update of n rows (after the ignore_index filter): the score dtype on its
+ * loop branch (binary: n > 50 000; multiclass: n * num_classes^2 > 10^6), else the promotion of score and threshold dtypes
+ * (multilabel always).  -1 for a score or threshold tag that is not accepted. */
+MB200_API int mb200_binned_curve_compare_dtype(int preds_dtype, int thresholds_dtype, int64_t n, int64_t num_classes,
+                                               int multilabel);
 MB200_API int mb200_binned_curve_update(const void* preds, int preds_dtype, const void* target, int target_dtype,
-                                        int64_t n, int64_t num_classes, const float* thresholds_sorted,
-                                        int64_t num_thresholds, int64_t* confmat, uint64_t* scratch, void* stream);
-/* Multilabel variant (replaces precision_recall_curve.py:777-799 _multilabel_precision_recall_curve_update): target is
- * [n, num_labels] like preds; entries whose target is neither 0 nor 1 (ignore_index) are skipped.
- * confmat: int64 [num_thresholds, num_labels, 2, 2]. */
+                                        int64_t n, int64_t num_classes, const void* thresholds_sorted, int thresholds_dtype,
+                                        int compare_dtype, int64_t num_thresholds, int64_t* confmat, uint64_t* scratch,
+                                        void* stream);
+/* Multilabel variant (replaces precision_recall_curve.py:745-799 _multilabel_precision_recall_curve_format + _update):
+ * target is [n, num_labels] like preds; entries whose target is neither 0 nor 1, or (has_ignore_index != 0) equals
+ * ignore_index reduced to the target dtype's width, are skipped.  confmat: int64 [num_thresholds, num_labels, 2, 2]. */
 MB200_API int mb200_binned_curve_update_multilabel(const void* preds, int preds_dtype, const void* target,
                                                    int target_dtype, int64_t n, int64_t num_labels,
-                                                   const float* thresholds_sorted, int64_t num_thresholds,
+                                                   const void* thresholds_sorted, int thresholds_dtype, int compare_dtype,
+                                                   int64_t num_thresholds, int has_ignore_index, int64_t ignore_index,
                                                    int64_t* confmat, uint64_t* scratch, void* stream);
 
 /* ------------------------------------------------------------------------------------------------

@@ -122,8 +122,9 @@ SIGNATURES = {
     "mb200_regression_scratch_doubles": ("q", "qqi"),
     "mb200_regression_sums": ("i", "ppiqqiddppp"),
     "mb200_binned_curve_scratch_words": ("q", "qq"),
-    "mb200_binned_curve_update": ("i", "pipiqqpqppp"),
-    "mb200_binned_curve_update_multilabel": ("i", "pipiqqpqppp"),
+    "mb200_binned_curve_compare_dtype": ("i", "iiqqi"),
+    "mb200_binned_curve_update": ("i", "pipiqqpiiqppp"),
+    "mb200_binned_curve_update_multilabel": ("i", "pipiqqpiiqiqppp"),
     "mb200_multiclass_stats_softmax_update": ("i", "pipiqqippppppppp"),
     "mb200_peer_pack_keys_put": ("i", "piqqqiqqpqp"),
     "mb200_peer_put_all": ("i", "pqpqip"),
@@ -784,14 +785,17 @@ def _is_sorted(thr: Tensor) -> bool:
 
 
 def binned_curve_update(preds: Tensor, target: Tensor, thresholds: Tensor, num_classes: int = 1,
-                        multilabel: bool = False) -> Tensor:
+                        multilabel: bool = False, ignore_index: Optional[int] = None) -> Tensor:
     """Multi-threshold confusion matrix of one batch: int64 ``[T, 2, 2]`` (``num_classes == 1``) or ``[T, C, 2, 2]``.
-    ``thresholds`` may be in any order (rows of the result follow it); the kernel works on a sorted copy.
-    ``multilabel``: ``target`` is ``[N, C]`` like ``preds``; entries that are neither 0 nor 1 are skipped."""
+    ``thresholds`` may be in any order (rows of the result follow it) and of any float or integer dtype: the kernel works on
+    a copy sorted in that dtype and compares ``score >= threshold`` in the dtype the reference would for this batch
+    (``mb200_binned_curve_compare_dtype``: the score dtype above its size rule, the promoted dtype below it).
+    ``multilabel``: ``target`` is ``[N, C]`` like ``preds``; entries that are neither 0 nor 1, or equal ``ignore_index`` in
+    the target's dtype, are skipped."""
     dev = require_cuda(preds, target, thresholds)
     preds = preds.contiguous()
     target = target.contiguous()
-    thr = thresholds.to(torch.float32)
+    thr = thresholds
     order = None
     if thr.numel() > 1 and not _is_sorted(thr):
         thr, order = torch.sort(thr)
@@ -801,12 +805,17 @@ def binned_curve_update(preds: Tensor, target: Tensor, thresholds: Tensor, num_c
     confmat = torch.zeros((t_count, num_classes, 2, 2), dtype=torch.int64, device=dev)
     lib_ = lib()
     scratch = torch.zeros(int(lib_.mb200_binned_curve_scratch_words(i64(num_classes), i64(t_count))), dtype=torch.int64, device=dev)
+    cmp = lib_.mb200_binned_curve_compare_dtype(tag(preds), tag(thr), n, num_classes, 1 if multilabel else 0)
     with on_device(dev):
-        fn = lib_.mb200_binned_curve_update_multilabel if multilabel else lib_.mb200_binned_curve_update
-        rc = fn(
-            ptr(preds), tag(preds), ptr(target), tag(target), i64(n), i64(num_classes), ptr(thr), i64(t_count),
-            ptr(confmat), ptr(scratch), stream_handle(dev),
-        )
+        if multilabel:
+            rc = lib_.mb200_binned_curve_update_multilabel(
+                ptr(preds), tag(preds), ptr(target), tag(target), i64(n), i64(num_classes), ptr(thr), tag(thr), cmp, i64(t_count),
+                0 if ignore_index is None else 1, 0 if ignore_index is None else int(ignore_index), ptr(confmat), ptr(scratch),
+                stream_handle(dev))
+        else:
+            rc = lib_.mb200_binned_curve_update(
+                ptr(preds), tag(preds), ptr(target), tag(target), i64(n), i64(num_classes), ptr(thr), tag(thr), cmp, i64(t_count),
+                ptr(confmat), ptr(scratch), stream_handle(dev))
     check(rc, "binned_curve_update")
     if order is not None:
         inv = torch.empty_like(order)

@@ -234,7 +234,7 @@ class MultilabelPrecisionRecallCurve(Metric):
         preds, target, _ = _multilabel_precision_recall_curve_format(
             preds, target, self.num_labels, self.thresholds, self.ignore_index
         )
-        state = _multilabel_precision_recall_curve_update(preds, target, self.num_labels, self.thresholds)
+        state = _multilabel_precision_recall_curve_update(preds, target, self.num_labels, self.thresholds, self.ignore_index)
         self._accumulate(state)
 
     def compute(self):

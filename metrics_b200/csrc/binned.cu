@@ -25,33 +25,78 @@ __device__ __forceinline__ float binned_to_float<double>(double x) { return (flo
 template <typename T>
 struct CmpType { using type = float; };
 template <>
-struct CmpType<double> { using type = double; };  // fp64 scores are compared against the fp32 thresholds in fp64
+struct CmpType<double> { using type = double; };  // fp64 scores are compared in fp64
 template <typename T>
 __device__ __forceinline__ typename CmpType<T>::type binned_load(const T* p, long long i) { return binned_to_float<T>(p[i]); }
 template <>
 __device__ __forceinline__ double binned_load<double>(const double* p, long long i) { return p[i]; }
 
+// Threshold i of a list of any float or integer dtype, exactly (integers up to 2^53).
+__device__ __forceinline__ double binned_threshold(const void* thr, int thr_dtype, long long i) {
+    switch (thr_dtype) {
+        case MB200_F32: return reinterpret_cast<const float*>(thr)[i];
+        case MB200_F16: return __half2float(reinterpret_cast<const __half*>(thr)[i]);
+        case MB200_BF16: return __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(thr)[i]);
+        case MB200_F64: return reinterpret_cast<const double*>(thr)[i];
+        default: return (double)load_label(thr, thr_dtype, i);
+    }
+}
+
+// The comparand c of threshold t for `score >= t` evaluated in dtype cmp_dtype (DESIGN §2 K4): for every score p of the
+// kernel's score type, `p >= c` in Cmp holds exactly when the reference's comparison does.
+//  * f16 / bf16: ATen casts t to the score dtype (through float, as c10::Half / c10::BFloat16 do) and compares;
+//  * f32: t rounded to float;
+//  * f64 with float scores: the least float >= t (round up), since a float p is >= t exactly when it is >= that float;
+//  * f64 with double scores (Cmp = double): t itself.
+// Every case is a monotone function of t, so an ascending list stays ascending.
+template <typename Cmp>
+__device__ __forceinline__ Cmp binned_comparand(const void* thr, int thr_dtype, int cmp_dtype, long long i) {
+    const double t = binned_threshold(thr, thr_dtype, i);
+    if constexpr (std::is_same<Cmp, double>::value) {
+        return t;
+    } else {
+        switch (cmp_dtype) {
+            case MB200_F16: return __half2float(__float2half_rn((float)t));
+            case MB200_BF16: return __bfloat162float(__float2bfloat16_rn((float)t));
+            case MB200_F64: return __double2float_ru(t);
+            default: return (float)t;
+        }
+    }
+}
+
+// The same, for threshold lists read from global memory inside the bucket search: kept out of line, so that the conversion
+// does not inflate the search loop of the common case (comparands staged in shared memory).
+template <typename Cmp>
+__device__ __noinline__ Cmp binned_comparand_global(const void* thr, int thr_dtype, int cmp_dtype, long long i) {
+    return binned_comparand<Cmp>(thr, thr_dtype, cmp_dtype, i);
+}
+
 // bucket counts: scratch[(c * 2 + y) * (T + 1) + k], zero on entry, self-cleaning (the folding CTA re-zeroes it)
 template <typename T>
 __global__ void __launch_bounds__(256) binned_bucket_kernel(const T* __restrict__ preds, const void* __restrict__ target,
-                                                            int tdtype, long long n, int C, const float* __restrict__ thr,
-                                                            int nthr, unsigned long long* __restrict__ scratch,
+                                                            int tdtype, long long n, int C, const void* __restrict__ thr,
+                                                            int thr_dtype, int cmp_dtype, int nthr,
+                                                            unsigned long long* __restrict__ scratch,
                                                             long long* __restrict__ confmat, int use_smem, int multilabel,
-                                                            int thr_in_smem) {
-    extern __shared__ unsigned sh_cnt[];  // [C * 2 * (nthr + 1) when use_smem] counters, then nthr thresholds
+                                                            int thr_in_smem, int has_ignore, long long ignore) {
+    // [C * 2 * (nthr + 1) when use_smem] counters, then nthr comparands (8-byte aligned: the counter count is even)
+    extern __shared__ __align__(8) unsigned sh_cnt[];
     const int stride = nthr + 1;
     const int ncnt = C * 2 * stride;
     typedef typename CmpType<T>::type Cmp;
-    float* sh_stage = reinterpret_cast<float*>(sh_cnt + (use_smem ? ncnt : 0));
+    Cmp* sh_stage = reinterpret_cast<Cmp*>(sh_cnt + (use_smem ? ncnt : 0));
     if (thr_in_smem)
-        for (int i = threadIdx.x; i < nthr; i += blockDim.x) sh_stage[i] = thr[i];
-    const float* __restrict__ sh_thr = thr_in_smem ? sh_stage : thr;  // very long threshold lists stay in global memory
+        for (int i = threadIdx.x; i < nthr; i += blockDim.x) sh_stage[i] = binned_comparand<Cmp>(thr, thr_dtype, cmp_dtype, i);
+    // very long threshold lists (or f64 ones next to large counters) stay in global memory and are converted per read
+    auto sh_thr = [&](int k) -> Cmp {
+        return thr_in_smem ? sh_stage[k] : binned_comparand_global<Cmp>(thr, thr_dtype, cmp_dtype, k);
+    };
     if (use_smem)
         for (int i = threadIdx.x; i < ncnt; i += blockDim.x) sh_cnt[i] = 0;
     __syncthreads();
     // bucket hint for (near-)uniform grids: k ~ (p - thr[0]) * (nthr - 1) / (thr[last] - thr[0]); the exact bucket is then
     // found by stepping against the real thresholds, so the hint only affects speed, never the result
-    const float t_first = sh_thr[0], t_last = sh_thr[nthr - 1];
+    const float t_first = (float)sh_thr(0), t_last = (float)sh_thr(nthr - 1);
     const float scale = (nthr > 1 && t_last > t_first) ? (float)(nthr - 1) / (t_last - t_first) : 0.f;
     const long long total = n * C;
     const bool flat = (C == 1) || multilabel;  // label index == element index
@@ -62,14 +107,14 @@ __global__ void __launch_bounds__(256) binned_bucket_kernel(const T* __restrict_
             const float h = ((float)p - t_first) * scale;
             k = h <= 0.f ? 0 : (h >= (float)nthr ? nthr : (int)h);
             int steps = 0;
-            while (k < nthr && (Cmp)sh_thr[k] <= p && steps < 4) ++k, ++steps;
-            while (k > 0 && !((Cmp)sh_thr[k - 1] <= p) && steps < 8) --k, ++steps;
-            const bool settled = (k == nthr || !((Cmp)sh_thr[k] <= p)) && (k == 0 || (Cmp)sh_thr[k - 1] <= p);
+            while (k < nthr && sh_thr(k) <= p && steps < 4) ++k, ++steps;
+            while (k > 0 && !(sh_thr(k - 1) <= p) && steps < 8) --k, ++steps;
+            const bool settled = (k == nthr || !(sh_thr(k) <= p)) && (k == 0 || sh_thr(k - 1) <= p);
             if (!settled) {  // irregular thresholds: plain binary search
                 int lo = 0, hi = nthr;
                 while (lo < hi) {
                     const int mid = (lo + hi) >> 1;
-                    if ((Cmp)sh_thr[mid] <= p) lo = mid + 1;
+                    if (sh_thr(mid) <= p) lo = mid + 1;
                     else hi = mid;
                 }
                 k = lo;
@@ -81,6 +126,7 @@ __global__ void __launch_bounds__(256) binned_bucket_kernel(const T* __restrict_
         // multilabel: target is [n, C] like preds, every label is its own binary problem
         const int y = (C == 1 || multilabel) ? (t == 1) : (t == c);
         if ((C == 1 || multilabel) && (unsigned long long)t > 1ull) return;  // binary: only {0,1} targets take part
+        if (has_ignore && t == ignore) return;                               // multilabel ignore_index (0 or 1)
         const int slot = (c * 2 + y) * stride + bucket_of(p);
         if (use_smem) atomicAdd(&sh_cnt[slot], 1u);
         else atomicAdd(&scratch[slot], 1ull);
@@ -178,7 +224,8 @@ __device__ __forceinline__ void load4_labels(const LabelT* __restrict__ t, unsig
 constexpr int kBinCells = 4096;
 template <typename LabelT>
 __global__ void __launch_bounds__(256) binned_binary_fast_kernel(const float* __restrict__ preds, const LabelT* __restrict__ target,
-                                                                 unsigned n, const float* __restrict__ thr, int nthr,
+                                                                 unsigned n, const void* __restrict__ thr, int thr_dtype,
+                                                                 int cmp_dtype, int nthr,
                                                                  unsigned long long* __restrict__ scratch,
                                                                  long long* __restrict__ confmat) {
     extern __shared__ unsigned sh_fast[];  // [2 * (nthr + 1)] counters | nthr thresholds | kBinCells cell table
@@ -186,7 +233,7 @@ __global__ void __launch_bounds__(256) binned_binary_fast_kernel(const float* __
     const int ncnt = 2 * stride;
     float* sh_thr = reinterpret_cast<float*>(sh_fast + ncnt);
     unsigned* cell = sh_fast + ncnt + nthr;  // per cell: low 16 bits = #thresholds in lower cells, high 16 = #thresholds inside
-    for (int i = threadIdx.x; i < nthr; i += blockDim.x) sh_thr[i] = thr[i];
+    for (int i = threadIdx.x; i < nthr; i += blockDim.x) sh_thr[i] = binned_comparand<float>(thr, thr_dtype, cmp_dtype, i);
     for (int i = threadIdx.x; i < ncnt; i += blockDim.x) sh_fast[i] = 0;
     for (int i = threadIdx.x; i < kBinCells; i += blockDim.x) cell[i] = 0;
     __syncthreads();
@@ -303,20 +350,38 @@ extern "C" int64_t mb200_binned_curve_scratch_words(int64_t num_classes, int64_t
     return num_classes * 2 * (num_thresholds + 1) + 8;
 }
 
+// The dtype D in which the reference evaluates `score >= threshold` for one update (DESIGN §2 K4).  Binary (and micro)
+// updates of more than 50 000 scores and multiclass updates with n * C * C > 10^6 take the reference's loop branch,
+// `preds >= thresholds[i]` with a 0-dim threshold: D is the score dtype.  Smaller ones and every multilabel update take
+// its vectorized branch, `preds.unsqueeze(-1) >= thresholds.unsqueeze(0)`: D is torch.promote_types(score, threshold).
+extern "C" int mb200_binned_curve_compare_dtype(int preds_dtype, int thresholds_dtype, int64_t n, int64_t num_classes,
+                                                int multilabel) {
+    if (!is_float_tag(preds_dtype) || !(is_float_tag(thresholds_dtype) || with_label_type(thresholds_dtype, [](auto) { return 0; }) == 0))
+        return -1;
+    const bool loop = !multilabel && (num_classes == 1 ? n > 50000 : (double)n * (double)num_classes * (double)num_classes > 1e6);
+    if (loop || !is_float_tag(thresholds_dtype) || thresholds_dtype == preds_dtype) return preds_dtype;
+    if (preds_dtype == MB200_F64 || thresholds_dtype == MB200_F64) return MB200_F64;
+    return MB200_F32;  // f32 with anything narrower, and f16 with bf16
+}
+
 static int binned_update_impl(int multilabel, const void* preds, int preds_dtype, const void* target, int target_dtype,
-                                         int64_t n, int64_t num_classes, const float* thresholds_sorted,
-                                         int64_t num_thresholds, int64_t* confmat, uint64_t* scratch, void* stream) {
+                              int64_t n, int64_t num_classes, const void* thresholds_sorted, int thr_dtype, int cmp_dtype,
+                              int64_t num_thresholds, int has_ignore, int64_t ignore_index, int64_t* confmat, uint64_t* scratch,
+                              void* stream) {
     MB200_REQUIRE(n >= 0 && num_classes >= 1 && num_thresholds >= 1, "bad sizes");
     MB200_REQUIRE(num_thresholds < (1 << 24) && num_classes < (1 << 24), "sizes too large");
     if (n == 0) return 0;
     MB200_REQUIRE(preds && target && thresholds_sorted && confmat && scratch, "NULL pointer");
     MB200_REQUIRE(is_float_tag(preds_dtype), "scores must be floating point (dtype tag %d)", preds_dtype);
+    MB200_REQUIRE(is_float_tag(thr_dtype) || with_label_type(thr_dtype, [](auto) { return 0; }) == 0,
+                  "thresholds must be floating point or integer (dtype tag %d)", thr_dtype);
+    MB200_REQUIRE(cmp_dtype == MB200_F64 || (cmp_dtype == MB200_F32 && preds_dtype != MB200_F64) || cmp_dtype == preds_dtype,
+                  "comparison dtype tag %d is not reachable from score dtype tag %d", cmp_dtype, preds_dtype);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const long long total = n * num_classes;
+    const long long ignore = has_ignore ? label_ignore_index(ignore_index, target_dtype) : 0;
     const size_t smem_need = (size_t)num_classes * 2 * (num_thresholds + 1) * sizeof(unsigned);
     const int use_smem = smem_need <= 40 * 1024;
-    const int thr_in_smem = num_thresholds <= 2048;
-    const size_t smem_total = (use_smem ? smem_need : 0) + (thr_in_smem ? (size_t)num_thresholds * sizeof(float) : 0);
     long long blocks = (total + 256 * 8 - 1) / (256 * 8);
     const long long cap = (long long)sm_count() * 8;
     if (blocks > cap) blocks = cap;
@@ -335,26 +400,33 @@ static int binned_update_impl(int multilabel, const void* preds, int preds_dtype
         if (fb > fcap) fb = fcap;
         if (fb < 1) fb = 1;
         const float* pf = reinterpret_cast<const float*>(preds);
+        const int nt = (int)num_thresholds;
         if (target_dtype == MB200_I64)
             binned_binary_fast_kernel<long long><<<(int)fb, 256, smem_fast, st>>>(pf, (const long long*)target, (unsigned)n,
-                                                                                 thresholds_sorted, (int)num_thresholds, sc, cm);
+                                                                                 thresholds_sorted, thr_dtype, cmp_dtype, nt, sc, cm);
         else if (target_dtype == MB200_I32)
             binned_binary_fast_kernel<int><<<(int)fb, 256, smem_fast, st>>>(pf, (const int*)target, (unsigned)n, thresholds_sorted,
-                                                                           (int)num_thresholds, sc, cm);
+                                                                           thr_dtype, cmp_dtype, nt, sc, cm);
         else if (target_dtype == MB200_I8)
             binned_binary_fast_kernel<signed char><<<(int)fb, 256, smem_fast, st>>>(pf, (const signed char*)target, (unsigned)n,
-                                                                                   thresholds_sorted, (int)num_thresholds, sc, cm);
+                                                                                   thresholds_sorted, thr_dtype, cmp_dtype, nt, sc, cm);
         else
             binned_binary_fast_kernel<unsigned char><<<(int)fb, 256, smem_fast, st>>>(pf, (const unsigned char*)target, (unsigned)n,
-                                                                                     thresholds_sorted, (int)num_thresholds, sc, cm);
+                                                                                     thresholds_sorted, thr_dtype, cmp_dtype, nt, sc, cm);
         count_launch();
         return check_cuda(cudaGetLastError(), "binned curve launch");
     }
     with_float_type(preds_dtype, [&](auto t) {
         using T = typename decltype(t)::type;
-        binned_bucket_kernel<T><<<(int)blocks, 256, smem_total, st>>>(reinterpret_cast<const T*>(preds), target, target_dtype, n,
-                                                                     (int)num_classes, thresholds_sorted, (int)num_thresholds, sc,
-                                                                     cm, use_smem, multilabel, thr_in_smem);
+        using Cmp = typename CmpType<T>::type;
+        // comparands in shared memory when they fit beside the counters under the 48 KB that needs no opt-in: always for
+        // float comparands (40 KB + 2048 * 4 B), not for 2048 double ones next to more than 32 KB of counters
+        const size_t thr_bytes = (size_t)num_thresholds * sizeof(Cmp);
+        const size_t cnt_bytes = use_smem ? smem_need : 0;
+        const int thr_in_smem = num_thresholds <= 2048 && cnt_bytes + thr_bytes <= 48 * 1024;
+        binned_bucket_kernel<T><<<(int)blocks, 256, cnt_bytes + (thr_in_smem ? thr_bytes : 0), st>>>(
+            reinterpret_cast<const T*>(preds), target, target_dtype, n, (int)num_classes, thresholds_sorted, thr_dtype, cmp_dtype,
+            (int)num_thresholds, sc, cm, use_smem, multilabel, thr_in_smem, has_ignore ? 1 : 0, ignore);
         return 0;
     });
     count_launch();
@@ -362,17 +434,20 @@ static int binned_update_impl(int multilabel, const void* preds, int preds_dtype
 }
 
 extern "C" int mb200_binned_curve_update(const void* preds, int preds_dtype, const void* target, int target_dtype,
-                                         int64_t n, int64_t num_classes, const float* thresholds_sorted,
-                                         int64_t num_thresholds, int64_t* confmat, uint64_t* scratch, void* stream) {
-    return binned_update_impl(0, preds, preds_dtype, target, target_dtype, n, num_classes, thresholds_sorted, num_thresholds,
-                              confmat, scratch, stream);
+                                         int64_t n, int64_t num_classes, const void* thresholds_sorted, int thresholds_dtype,
+                                         int compare_dtype, int64_t num_thresholds, int64_t* confmat, uint64_t* scratch,
+                                         void* stream) {
+    return binned_update_impl(0, preds, preds_dtype, target, target_dtype, n, num_classes, thresholds_sorted, thresholds_dtype,
+                              compare_dtype, num_thresholds, 0, 0, confmat, scratch, stream);
 }
 
-// multilabel: target is [n, num_labels] like preds; entries whose target is not 0 / 1 (e.g. ignore_index) are skipped
+// multilabel: target is [n, num_labels] like preds; entries whose target is not 0 / 1, or equals ignore_index reduced to the
+// target dtype's width, are skipped
 extern "C" int mb200_binned_curve_update_multilabel(const void* preds, int preds_dtype, const void* target,
                                                     int target_dtype, int64_t n, int64_t num_labels,
-                                                    const float* thresholds_sorted, int64_t num_thresholds,
+                                                    const void* thresholds_sorted, int thresholds_dtype, int compare_dtype,
+                                                    int64_t num_thresholds, int has_ignore_index, int64_t ignore_index,
                                                     int64_t* confmat, uint64_t* scratch, void* stream) {
-    return binned_update_impl(1, preds, preds_dtype, target, target_dtype, n, num_labels, thresholds_sorted, num_thresholds,
-                              confmat, scratch, stream);
+    return binned_update_impl(1, preds, preds_dtype, target, target_dtype, n, num_labels, thresholds_sorted, thresholds_dtype,
+                              compare_dtype, num_thresholds, has_ignore_index, ignore_index, confmat, scratch, stream);
 }

@@ -154,21 +154,28 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tenso
     return {auroc, ap, counts, fps, tps, thr};
 }
 
-// precision_recall_curve.py:191-251, 464-533, 777-799
+// precision_recall_curve.py:191-251, 464-533, 745-799; thresholds ascending, of any float or integer dtype
 void binned_curve_update_(at::Tensor& confmat, at::Tensor& scratch, const at::Tensor& preds, const at::Tensor& target,
-                          const at::Tensor& thresholds, int64_t num_classes, bool multilabel) {
+                          const at::Tensor& thresholds, int64_t num_classes, bool multilabel, c10::optional<int64_t> ignore_index) {
     same_cuda(confmat, {&scratch, &preds, &target, &thresholds});
     TORCH_CHECK(confmat.scalar_type() == at::kLong && confmat.is_contiguous() && scratch.scalar_type() == at::kLong &&
-                    thresholds.scalar_type() == at::kFloat && thresholds.is_contiguous(),
-                "confmat / scratch must be int64, thresholds float32, all contiguous");
+                    thresholds.is_contiguous(),
+                "confmat / scratch must be int64, all contiguous");
     TORCH_CHECK(scratch.numel() >= mb200_binned_curve_scratch_words(num_classes, thresholds.numel()), "scratch too small");
     const c10::cuda::CUDAGuard guard(confmat.device());
     const at::Tensor p = preds.contiguous(), t = target.contiguous();
     const int64_t n = multilabel || num_classes == 1 ? (num_classes == 1 ? p.numel() : p.size(0)) : p.size(0);
-    auto fn = multilabel ? mb200_binned_curve_update_multilabel : mb200_binned_curve_update;
-    ok(fn(p.data_ptr(), dtype_tag(p), t.data_ptr(), dtype_tag(t), n, num_classes, thresholds.data_ptr<float>(), thresholds.numel(),
-          confmat.data_ptr<int64_t>(), reinterpret_cast<uint64_t*>(scratch.data_ptr()), stream_of(confmat)),
-       "binned_curve_update_");
+    const int thr_tag = dtype_tag(thresholds);
+    const int cmp = mb200_binned_curve_compare_dtype(dtype_tag(p), thr_tag, n, num_classes, multilabel ? 1 : 0);
+    const int rc = multilabel
+        ? mb200_binned_curve_update_multilabel(p.data_ptr(), dtype_tag(p), t.data_ptr(), dtype_tag(t), n, num_classes,
+                                               thresholds.data_ptr(), thr_tag, cmp, thresholds.numel(), ignore_index.has_value(),
+                                               ignore_index.value_or(0), confmat.data_ptr<int64_t>(),
+                                               reinterpret_cast<uint64_t*>(scratch.data_ptr()), stream_of(confmat))
+        : mb200_binned_curve_update(p.data_ptr(), dtype_tag(p), t.data_ptr(), dtype_tag(t), n, num_classes, thresholds.data_ptr(),
+                                    thr_tag, cmp, thresholds.numel(), confmat.data_ptr<int64_t>(),
+                                    reinterpret_cast<uint64_t*>(scratch.data_ptr()), stream_of(confmat));
+    ok(rc, "binned_curve_update_");
 }
 
 // functional/regression/*.py `_x_update`: float64 [num_sums, num_outputs]
@@ -201,7 +208,7 @@ TORCH_LIBRARY(metrics_b200, m) {
     m.def("curve_evaluate(Tensor preds, Tensor target, int num_classes=1, int pos_label=1, bool want_curve=False) -> "
           "(Tensor auroc, Tensor ap, Tensor counts, Tensor fps, Tensor tps, Tensor thresholds)");
     m.def("binned_curve_update_(Tensor(a!) confmat, Tensor(b!) scratch, Tensor preds, Tensor target, Tensor thresholds, "
-          "int num_classes=1, bool multilabel=False) -> ()");
+          "int num_classes=1, bool multilabel=False, int? ignore_index=None) -> ()");
     m.def("regression_sums(Tensor preds, Tensor target, int op, int num_outputs=1, float param=0.0, float eps=0.0) -> Tensor");
 }
 

@@ -228,7 +228,7 @@ def _make_multilabel(kind: str) -> Callable:
             _floor_validation(fam.arg, floor)
             _multilabel_precision_recall_curve_tensor_validation(preds, target, num_labels, ignore_index)
         preds, target, thresholds = _multilabel_precision_recall_curve_format(preds, target, num_labels, thresholds, ignore_index)
-        state = _multilabel_precision_recall_curve_update(preds, target, num_labels, thresholds)
+        state = _multilabel_precision_recall_curve_update(preds, target, num_labels, thresholds, ignore_index)
         return _multilabel_at_fixed_compute(kind, state, num_labels, thresholds, ignore_index, floor)
 
     fn_.__name__ = fn_.__qualname__ = f"multilabel_{kind}"

@@ -204,7 +204,7 @@ def multilabel_average_precision(
         _multilabel_average_precision_arg_validation(num_labels, average, thresholds, ignore_index)
         _multilabel_precision_recall_curve_tensor_validation(preds, target, num_labels, ignore_index)
     preds, target, thresholds = _multilabel_precision_recall_curve_format(preds, target, num_labels, thresholds, ignore_index)
-    state = _multilabel_precision_recall_curve_update(preds, target, num_labels, thresholds)
+    state = _multilabel_precision_recall_curve_update(preds, target, num_labels, thresholds, ignore_index)
     return _multilabel_average_precision_compute(state, num_labels, average, thresholds, ignore_index)
 
 

@@ -382,7 +382,8 @@ def _multilabel_precision_recall_curve_format(
 ) -> tuple[Tensor, Tensor, Optional[Tensor]]:
     """``[N, L, ...] -> [N', L]``, sigmoid if the batch holds logits — reference :745-774.  Ignored entries stay in the
     state (they are dropped per label by the kernels: exact mode gives them the largest sort key, the binned kernel skips
-    every target that is neither 0 nor 1), so no masked copy of the batch is made."""
+    targets equal to ``ignore_index`` in the target's dtype and every target that is neither 0 nor 1), so no masked copy of
+    the batch is made."""
     preds = preds.transpose(0, 1).reshape(num_labels, -1).T
     target = target.transpose(0, 1).reshape(num_labels, -1).T
     preds = _native.sigmoid_if_logits(preds.contiguous())
@@ -390,13 +391,34 @@ def _multilabel_precision_recall_curve_format(
 
 
 def _multilabel_precision_recall_curve_update(
-    preds: Tensor, target: Tensor, num_labels: int, thresholds: Optional[Tensor]
+    preds: Tensor, target: Tensor, num_labels: int, thresholds: Optional[Tensor], ignore_index: Optional[int] = None
 ) -> Union[Tensor, tuple[Tensor, Tensor]]:
     """Exact mode keeps the batch; binned mode returns the ``[T, L, 2, 2]`` multi-threshold confusion matrix
-    (reference :777-799) from the K4 kernel."""
+    (reference :777-799) from the K4 kernel, which drops the entries the reference's format masks (``target ==
+    ignore_index``, :766-772) — also when ``ignore_index`` is 0 or 1."""
     if thresholds is None:
         return preds, target
-    return _native.binned_curve_update(preds, target, thresholds.to(preds.device), num_labels, multilabel=True)
+    # the kernel skips every target that is neither 0 nor 1 by itself: it is handed `ignore_index` only when that names label
+    # 0 or 1 in the target's dtype
+    extra = {"ignore_index": ignore_index} if _ignores_a_binary_label(ignore_index, target.dtype) else {}
+    return _native.binned_curve_update(preds, target, thresholds.to(preds.device), num_labels, multilabel=True, **extra)
+
+
+_LABEL_WIDTH = {torch.uint8: (8, False), torch.int8: (8, True), torch.int16: (16, True), torch.int32: (32, True)}
+
+
+def _ignores_a_binary_label(ignore_index: Optional[int], dtype: torch.dtype) -> bool:
+    """Does ``target == ignore_index`` select targets holding 0 or 1?  ATen casts the Python int to the target's dtype
+    first (two's complement wrap: with uint8 targets 257 is 1); int64 and bool targets compare the value itself."""
+    if ignore_index is None:
+        return False
+    v = int(ignore_index)
+    if dtype in _LABEL_WIDTH:
+        width, signed = _LABEL_WIDTH[dtype]
+        v &= (1 << width) - 1
+        if signed and v >= 1 << (width - 1):
+            v -= 1 << width
+    return v in (0, 1)
 
 
 def _multilabel_curves(preds: Tensor, target: Tensor, num_labels: int, ignore_index: Optional[int]):
@@ -445,7 +467,7 @@ def multilabel_precision_recall_curve(
         _multilabel_precision_recall_curve_arg_validation(num_labels, thresholds, ignore_index)
         _multilabel_precision_recall_curve_tensor_validation(preds, target, num_labels, ignore_index)
     preds, target, thresholds = _multilabel_precision_recall_curve_format(preds, target, num_labels, thresholds, ignore_index)
-    state = _multilabel_precision_recall_curve_update(preds, target, num_labels, thresholds)
+    state = _multilabel_precision_recall_curve_update(preds, target, num_labels, thresholds, ignore_index)
     return _multilabel_precision_recall_curve_compute(state, num_labels, thresholds, ignore_index)
 
 

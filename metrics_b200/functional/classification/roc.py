@@ -186,7 +186,7 @@ def multilabel_roc(
         _multilabel_precision_recall_curve_arg_validation(num_labels, thresholds, ignore_index)
         _multilabel_precision_recall_curve_tensor_validation(preds, target, num_labels, ignore_index)
     preds, target, thresholds = _multilabel_precision_recall_curve_format(preds, target, num_labels, thresholds, ignore_index)
-    state = _multilabel_precision_recall_curve_update(preds, target, num_labels, thresholds)
+    state = _multilabel_precision_recall_curve_update(preds, target, num_labels, thresholds, ignore_index)
     return _multilabel_roc_compute(state, num_labels, thresholds, ignore_index)
 
 

@@ -93,7 +93,7 @@ def _register_fakes() -> None:
                 torch.empty((num_classes, n), **f32), torch.empty((num_classes, n), dtype=thr_dtype, device=preds.device))
 
     @fake("metrics_b200::binned_curve_update_")
-    def _(confmat, scratch, preds, target, thresholds, num_classes=1, multilabel=False):
+    def _(confmat, scratch, preds, target, thresholds, num_classes=1, multilabel=False, ignore_index=None):
         return None
 
     @fake("metrics_b200::regression_sums")

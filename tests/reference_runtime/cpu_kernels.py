@@ -287,14 +287,18 @@ def regression_sums(preds, target, op, num_outputs=1, param=0.0, eps=0.0) -> Ten
     return torch.stack([x.double().sum(0) for x in terms])
 
 
-def binned_curve_update(preds, target, thresholds, num_classes=1, multilabel=False) -> Tensor:
-    thr = thresholds.to(torch.float32)
+def binned_curve_update(preds, target, thresholds, num_classes=1, multilabel=False, ignore_index=None) -> Tensor:
+    """`score >= threshold` in the dtype `mb200_binned_curve_compare_dtype` picks: the score dtype above the reference's
+    size rule (its loop branch), the promoted dtype below it and for multilabel (its vectorized branch)."""
+    n = preds.shape[0] if multilabel else target.numel()
+    loop = not multilabel and (n > 50_000 if num_classes == 1 else n * num_classes * num_classes > 1_000_000)
+    cmp_dtype = preds.dtype if loop else torch.promote_types(preds.dtype, thresholds.dtype)
+    thr = thresholds.to(cmp_dtype)
     t_count = thr.numel()
-    cmp_dtype = torch.float64 if preds.dtype == torch.float64 else torch.float32
     if num_classes == 1 and not multilabel:
         p, t = preds.reshape(-1).to(cmp_dtype), target.reshape(-1)
         out = torch.zeros((t_count, 2, 2), dtype=torch.int64)
-        ge = p[:, None] >= thr.to(cmp_dtype)[None, :]
+        ge = p[:, None] >= thr[None, :]
         for y in (0, 1):
             sel = t == y
             out[:, y, 1] = ge[sel].sum(0)
@@ -303,9 +307,11 @@ def binned_curve_update(preds, target, thresholds, num_classes=1, multilabel=Fal
     out = torch.zeros((t_count, num_classes, 2, 2), dtype=torch.int64)
     for c in range(num_classes):
         p = preds[:, c].to(cmp_dtype)
-        ge = p[:, None] >= thr.to(cmp_dtype)[None, :]
+        ge = p[:, None] >= thr[None, :]
         for y in (0, 1):
             sel = (target[:, c] == y) if multilabel else ((target == c) == bool(y))
+            if multilabel and ignore_index is not None:
+                sel &= target[:, c] != ignore_index
             out[:, c, y, 1] = ge[sel].sum(0)
             out[:, c, y, 0] = sel.sum() - out[:, c, y, 1]
     return out

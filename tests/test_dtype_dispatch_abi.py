@@ -94,10 +94,18 @@ ENTRIES = {
     "argmax": (FLOAT, INVALID, CLASS_DIM_MSG, lambda L, b, d: L.mb200_argmax_rows(b.p, d, N, C, 1, b.out, 0)),
     "stats_softmax": (FLOAT_NO_F64, INVALID, SCORES3_MSG, lambda L, b, d: L.mb200_multiclass_stats_softmax_update(
         b.p, d, b.t, I64, N, C, 0, b.tp, b.fp, b.tn, b.fn, b.ws, b.out, b.flag, b.err, 0)),
-    "binned": (FLOAT, INVALID, FLOAT_MSG,
-               lambda L, b, d: L.mb200_binned_curve_update(b.p, d, b.t, I64, N, 1, b.thr, 5, b.out, b.ws, 0)),
-    "binned_multilabel": (FLOAT, INVALID, FLOAT_MSG,
-                          lambda L, b, d: L.mb200_binned_curve_update_multilabel(b.p, d, b.t, I64, N, C, b.thr, 5, b.out, b.ws, 0)),
+    # K4 with float32 thresholds compared in float64, and (multilabel) uint8-wrapped ignore_index 257
+    "binned_dtypes": (FLOAT, INVALID, FLOAT_MSG,
+                      lambda L, b, d: L.mb200_binned_curve_update(b.p, d, b.t, I64, N, 1, b.thr, F32, F64, 5, b.out, b.ws, 0)),
+    "binned_multilabel_dtypes": (FLOAT, INVALID, FLOAT_MSG, lambda L, b, d: L.mb200_binned_curve_update_multilabel(
+        b.p, d, b.t, I64, N, C, b.thr, F32, F64, 5, 1, 257, b.out, b.ws, 0)),
+    # the thresholds' tag is the one varied: any float or integer list
+    "binned_thresholds": (FLOAT | LABELS - {_native.BOOL}, INVALID, "thresholds must be floating point or integer (dtype tag %d)",
+                          lambda L, b, d: L.mb200_binned_curve_update(b.p, F32, b.t, I64, N, 1, b.thr, d, F64, 5, b.out, b.ws, 0)),
+    "binned_multilabel_thresholds": (FLOAT | LABELS - {_native.BOOL}, INVALID,
+                                     "thresholds must be floating point or integer (dtype tag %d)",
+                                     lambda L, b, d: L.mb200_binned_curve_update_multilabel(
+                                         b.p, F32, b.t, I64, N, C, b.thr, d, F64, 5, 0, 0, b.out, b.ws, 0)),
     "kl_divergence": (FLOAT, INVALID, "distributions must be f32/f16/bf16/f64 (dtype tag %d)",
                       lambda L, b, d: L.mb200_kl_divergence_rows(b.p, b.t, d, N, C, 0, b.out, 0)),
     "peer_pack_keys_put": (FLOAT_NO_F64, INVALID, SCORES3_MSG,
