@@ -161,9 +161,20 @@ SIGNATURES = {
 }
 
 
+# include/mb200_image.h (K20), outside the include/metrics_b200*.h set until it joins the one drive table of
+# tests/test_abi.py; tests/test_image_abi.py checks it
+_VOL = "pipi" + "q" * 15  # preds, its tag, target, its tag, [b, c, d, h, w], preds strides, target strides
+IMAGE_SIGNATURES = {
+    "mb200_ssim_scratch_bytes": ("q", "iqqqqqiiiiii"),
+    "mb200_ssim_data_range": ("i", _VOL + "ddppqp"),
+    "mb200_ssim_update": ("i", _VOL + "iiiiiiipiddpddppppqp"),
+    "mb200_ssim_avg_pool": ("i", _VOL + "ippp"),
+}
+
+
 def declare_signatures(handle) -> None:
     """Set ``restype`` / ``argtypes`` of every exported function on a loaded library handle."""
-    for name, (ret, args) in SIGNATURES.items():
+    for name, (ret, args) in {**SIGNATURES, **IMAGE_SIGNATURES}.items():
         fn = getattr(handle, name)
         fn.restype = _C_TYPES[ret]
         fn.argtypes = [_C_TYPES[a] for a in args]
@@ -1407,3 +1418,87 @@ def hausdorff_distance(preds: Tensor, target: Tensor, num_classes: int, index_fo
     if rc:
         check(rc, "hausdorff_distance")
     return out, err
+
+
+# ----------------------------------------------------------------------------------------------------------
+# K20 wrappers (structural similarity, include/mb200_image.h)
+# ----------------------------------------------------------------------------------------------------------
+SSIM_RANGE, SSIM_C1, SSIM_C2, SSIM_CONSTS = 0, 1, 2, 3
+SSIM_MAX_TAPS = 255
+
+
+def _volume(x: Tensor) -> tuple[tuple, tuple]:
+    """``[b, c, d, h, w]`` and element strides of a 4-D (``d = 1``) or 5-D tensor, read in place."""
+    if x.ndim == 4:
+        (b, c, h, w), (sn, sc, sh, sw) = x.shape, x.stride()
+        return (b, c, 1, h, w), (sn, sc, 0, sh, sw)
+    return tuple(x.shape), tuple(x.stride())
+
+
+def ssim_scratch_bytes(preds: Tensor, taps: tuple, pads: tuple) -> int:
+    shape, _ = _volume(preds)
+    return int(lib().mb200_ssim_scratch_bytes(tag(preds), *shape, *taps, *pads))
+
+
+def ssim(preds: Tensor, target: Tensor, weights: Tensor, taps: tuple, pads: tuple, crop_depth: bool,
+         clamp: Optional[tuple], data_range: Optional[float], k1: float, k2: float, want_cs: bool,
+         want_map: bool) -> tuple[Tensor, Optional[Tensor], Optional[Tensor]]:
+    """K20: per-image float64 SSIM ``[b]``, the contrast term ``[b]`` over the crop (``want_cs``) and the map
+    ``[b, c, o_d, o_h, o_w]`` in ``preds``' dtype (``want_map``).  ``taps`` / ``pads``: per axis (d, h, w); ``weights``:
+    the ``sum(taps)`` filter taps in ``preds``' dtype.  ``data_range=None`` runs the data-range pre-pass first; its
+    constants stay on the device.  ``target`` of any float dtype is rounded to ``preds``' dtype on load.  No host
+    synchronisation."""
+    dev = require_cuda(preds, target, weights)
+    shape, ps = _volume(preds)
+    _, ts = _volume(target)
+    b = shape[0]
+    lib_ = lib()
+    nbytes = int(lib_.mb200_ssim_scratch_bytes(tag(preds), *shape, *taps, *pads))
+    if nbytes < 0:
+        raise ValueError(f"metrics_b200: a filter of {tuple(taps)} taps with pads {tuple(pads)} on {tuple(shape[2:])} "
+                         f"needs more than one CTA's shared memory or gives an empty output, or the batch of {shape[0]} x "
+                         f"{shape[1]} planes needs 2^31 tiles or more")
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    sim = torch.empty(b, dtype=torch.float64, device=dev)
+    cs = torch.empty(b, dtype=torch.float64, device=dev) if want_cs else None
+    out_shape = (shape[0], shape[1], *(n + 2 * p - k + 1 for n, p, k in zip(shape[2:], pads, taps)))
+    img = torch.empty(out_shape, dtype=preds.dtype, device=dev) if want_map else None
+    stream = stream_handle(dev)
+    consts = None
+    with on_device(dev):
+        if data_range is None:
+            consts = torch.empty(SSIM_CONSTS, dtype=torch.float64, device=dev)
+            rc = lib_.mb200_ssim_data_range(preds.data_ptr(), tag(preds), target.data_ptr(), tag(target), *shape, *ps, *ts,
+                                            float(k1), float(k2), consts.data_ptr(), scratch.data_ptr(), nbytes, stream)
+            if rc:
+                check(rc, "ssim_data_range")
+            c1 = c2 = 0.0
+        else:
+            c1, c2 = (k1 * data_range) ** 2, (k2 * data_range) ** 2
+        lo, hi = clamp if clamp is not None else (0.0, 0.0)
+        rc = lib_.mb200_ssim_update(
+            preds.data_ptr(), tag(preds), target.data_ptr(), tag(target), *shape, *ps, *ts, *taps, *pads,
+            int(bool(crop_depth)), weights.data_ptr(), int(clamp is not None), float(lo), float(hi), ptr(consts),
+            float(c1), float(c2), sim.data_ptr(), ptr(cs), ptr(img), scratch.data_ptr(), nbytes, stream)
+    if rc:
+        check(rc, "ssim_update")
+    return sim, cs, img
+
+
+def ssim_avg_pool(preds: Tensor, target: Tensor, pool_depth: bool) -> tuple[Tensor, Tensor]:
+    """The next MS-SSIM scale of both inputs: 2x2 (2-D) or 2x2x2 (``pool_depth``) average pool, floor sizes,
+    contiguous in ``preds``' dtype (``target`` rounded to it first), shaped as the inputs' rank."""
+    dev = require_cuda(preds, target)
+    shape, ps = _volume(preds)
+    _, ts = _volume(target)
+    out = list(preds.shape[:2]) + [n // 2 for n in preds.shape[2:]]
+    if not pool_depth and preds.ndim == 5:
+        out[2] = preds.shape[2]
+    po = torch.empty(out, dtype=preds.dtype, device=dev)
+    to = torch.empty(out, dtype=preds.dtype, device=dev)
+    with on_device(dev):
+        rc = lib().mb200_ssim_avg_pool(preds.data_ptr(), tag(preds), target.data_ptr(), tag(target), *shape, *ps, *ts,
+                                       int(bool(pool_depth)), po.data_ptr(), to.data_ptr(), stream_handle(dev))
+    if rc:
+        check(rc, "ssim_avg_pool")
+    return po, to
