@@ -161,7 +161,7 @@ SIGNATURES = {
 }
 
 
-# include/mb200_image.h (K20), outside the include/metrics_b200*.h set until it joins the one drive table of
+# include/mb200_image.h (K20, K21), outside the include/metrics_b200*.h set until it joins the one drive table of
 # tests/test_abi.py; tests/test_image_abi.py checks it
 _VOL = "pipi" + "q" * 15  # preds, its tag, target, its tag, [b, c, d, h, w], preds strides, target strides
 IMAGE_SIGNATURES = {
@@ -169,6 +169,9 @@ IMAGE_SIGNATURES = {
     "mb200_ssim_data_range": ("i", _VOL + "ddppqp"),
     "mb200_ssim_update": ("i", _VOL + "iiiiiiipiddpddppppqp"),
     "mb200_ssim_avg_pool": ("i", _VOL + "ippp"),
+    "mb200_vif_scale_update": ("i", _VOL + "iiipddpppqp"),
+    "mb200_vif_decimate": ("i", _VOL + "iipppp"),
+    "mb200_uqi_update": ("i", _VOL + "iiiiiiiipdpppqp"),
 }
 
 
@@ -1502,3 +1505,73 @@ def ssim_avg_pool(preds: Tensor, target: Tensor, pool_depth: bool) -> tuple[Tens
     if rc:
         check(rc, "ssim_avg_pool")
     return po, to
+
+
+# ----------------------------------------------------------------------------------------------------------
+# K21 wrappers (VIF and UQI on K20's moments, include/mb200_image.h)
+# ----------------------------------------------------------------------------------------------------------
+def _moment_scratch(preds: Tensor, shape: tuple, taps: tuple, pads: tuple, dev) -> tuple[Tensor, int]:
+    nbytes = int(lib().mb200_ssim_scratch_bytes(tag(preds), *shape, *taps, *pads))
+    if nbytes < 0:
+        raise ValueError(f"metrics_b200: a filter of {tuple(taps)} taps with pads {tuple(pads)} on {tuple(shape[2:])} "
+                         f"needs more than one CTA's shared memory or gives an empty output, or the batch of {shape[0]} x "
+                         f"{shape[1]} planes needs 2^31 tiles or more")
+    return torch.empty(nbytes, dtype=torch.uint8, device=dev), nbytes
+
+
+def vif_scale(preds: Tensor, target: Tensor, weights: Tensor, taps: tuple, eps: float,
+              sigma_n_sq: float) -> tuple[Tensor, Tensor]:
+    """K21, one VIF scale with valid filtering: float64 ``[b, c]`` sums of the preds term and of the target term.
+    ``taps``: per axis (d, h, w); ``weights``: the ``sum(taps)`` taps in ``preds``' dtype; ``eps`` and ``sigma_n_sq``
+    already rounded to that dtype.  No host synchronisation."""
+    dev = require_cuda(preds, target, weights)
+    shape, ps = _volume(preds)
+    _, ts = _volume(target)
+    scratch, nbytes = _moment_scratch(preds, shape, taps, (0, 0, 0), dev)
+    sums = torch.empty(2, shape[0], shape[1], dtype=torch.float64, device=dev)
+    with on_device(dev):
+        rc = lib().mb200_vif_scale_update(
+            preds.data_ptr(), tag(preds), target.data_ptr(), tag(target), *shape, *ps, *ts, *taps, weights.data_ptr(),
+            float(eps), float(sigma_n_sq), sums[0].data_ptr(), sums[1].data_ptr(), scratch.data_ptr(), nbytes,
+            stream_handle(dev))
+    if rc:
+        check(rc, "vif_scale_update")
+    return sums[0], sums[1]
+
+
+def vif_decimate(preds: Tensor, target: Tensor, weights: Tensor, taps: tuple) -> tuple[Tensor, Tensor]:
+    """``conv2d(x, k)[..., ::2, ::2]`` of both 4-D inputs with the separable filter ``weights`` (``taps = (h, w)``),
+    contiguous in ``preds``' dtype."""
+    dev = require_cuda(preds, target, weights)
+    shape, ps = _volume(preds)
+    _, ts = _volume(target)
+    out = (*preds.shape[:2], (preds.shape[2] - taps[0] + 2) // 2, (preds.shape[3] - taps[1] + 2) // 2)
+    po = torch.empty(out, dtype=preds.dtype, device=dev)
+    to = torch.empty(out, dtype=preds.dtype, device=dev)
+    with on_device(dev):
+        rc = lib().mb200_vif_decimate(preds.data_ptr(), tag(preds), target.data_ptr(), tag(target), *shape, *ps, *ts,
+                                      *taps, weights.data_ptr(), po.data_ptr(), to.data_ptr(), stream_handle(dev))
+    if rc:
+        check(rc, "vif_decimate")
+    return po, to
+
+
+def uqi(preds: Tensor, target: Tensor, weights: Tensor, taps: tuple, pads: tuple, crop: tuple, eps: float,
+        want_map: bool) -> tuple[Tensor, Optional[Tensor]]:
+    """K21, UQI: per-image float64 sums ``[b]`` of the map over the crop ``[crop_h : o_h - crop_h] x
+    [crop_w : o_w - crop_w]``, and the full map ``[b, c, o_d, o_h, o_w]`` in ``preds``' dtype (``want_map``).  ``taps``
+    / ``pads``: per axis (d, h, w), reflect pads.  No host synchronisation."""
+    dev = require_cuda(preds, target, weights)
+    shape, ps = _volume(preds)
+    _, ts = _volume(target)
+    scratch, nbytes = _moment_scratch(preds, shape, taps, pads, dev)
+    sums = torch.empty(shape[0], dtype=torch.float64, device=dev)
+    out_shape = (shape[0], shape[1], *(n + 2 * p - k + 1 for n, p, k in zip(shape[2:], pads, taps)))
+    img = torch.empty(out_shape, dtype=preds.dtype, device=dev) if want_map else None
+    with on_device(dev):
+        rc = lib().mb200_uqi_update(
+            preds.data_ptr(), tag(preds), target.data_ptr(), tag(target), *shape, *ps, *ts, *taps, *pads, *crop,
+            weights.data_ptr(), float(eps), sums.data_ptr(), ptr(img), scratch.data_ptr(), nbytes, stream_handle(dev))
+    if rc:
+        check(rc, "uqi_update")
+    return sums, img

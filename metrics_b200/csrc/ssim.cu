@@ -2,6 +2,9 @@
 // functionals) on sm_90a: one read of preds and target per scale, the five windowed moments of a separable filter in
 // shared memory, the reference's epilogue, and per-image float64 means in a fixed order.
 //
+// K21 — VisualInformationFidelity and UniversalImageQualityIndex on the same moment kernel with their own epilogues
+// (functional/image/vif.py:45-83, functional/image/uqi.py:87-116), and the decimation between VIF scales.
+//
 // Reference op chain replaced (src/torchmetrics/functional/image/ssim.py):
 //   :113-121   data range (Python max of two tensor ranges, a host synchronisation), tuple clamp, c1 / c2
 //   :135-150   reflect padding of both inputs, gaussian / uniform kernel
@@ -146,11 +149,98 @@ __device__ __forceinline__ double warp_sum(double v) {
     return v;
 }
 
-// grid: one CTA per (image, channel, output depth, tile row, tile column), in that order, slowest first
-template <typename T, int TH>
-__global__ void __launch_bounds__(kThreads) ssim_kernel(Vol P, Vol Q, Geo g, const T* __restrict__ weights, Clamp cl,
-                                                        const double* __restrict__ consts, double c1_arg, double c2_arg,
-                                                        T* __restrict__ map, double2* __restrict__ partials) {
+// ---- epilogues: what ssim_kernel makes of the moments of one output position ---------------------------------------
+// begin() runs once per CTA on its own copy; operator() takes the means, the clamped variances and the covariance of
+// one position and returns the map value and two float64 addends for the CTA's sums.
+template <typename A>
+struct EpiOut {
+    A map;
+    double s0, s1;
+};
+
+// SSIM: the map into s0; upper / lower inside the crop [pad : o − pad] of every axis (and depth when crop_depth) into s1
+template <typename A>
+struct SsimEpilogue {
+    const double* consts;  // device [MB200_SSIM_CONSTS] of the data-range pass, or NULL for c1_arg / c2_arg
+    double c1_arg, c2_arg;
+    A c1, c2;
+    bool depth_in_crop;
+
+    __device__ __forceinline__ void begin(const Geo& g, long long od) {
+        if (consts) {
+            c1 = (A)consts[MB200_SSIM_C1];
+            c2 = (A)consts[MB200_SSIM_C2];
+        } else {
+            c1 = (A)c1_arg;
+            c2 = (A)c2_arg;
+        }
+        depth_in_crop = !g.crop_depth || (g.pd > 0 && od >= g.pd && od < g.od - g.pd);
+    }
+    __device__ __forceinline__ EpiOut<A> operator()(A mux, A muy, A vx, A vy, A cxy, const Geo& g, long long oh,
+                                                    long long ow) const {
+        const A upper = (A)2 * cxy + c2;
+        const A lower = (vx + vy) + c2;
+        const A s = (((A)2 * (mux * muy) + c1) * upper) / ((mux * mux + muy * muy + c1) * lower);
+        const bool in_crop =
+            depth_in_crop && g.ph > 0 && g.pw > 0 && oh >= g.ph && oh < g.oh - g.ph && ow >= g.pw && ow < g.ow - g.pw;
+        return {s, (double)s, in_crop ? (double)(upper / lower) : 0.0};
+    }
+};
+
+// UQI (functional/image/uqi.py:101-114): SSIM with c1 = c2 = 0 and the dtype's eps in the denominator; the map inside
+// the crop [crop_h : o_h − crop_h] x [crop_w : o_w − crop_w] into s0 (a zero margin is an empty crop, as x[0:-0])
+template <typename A>
+struct UqiEpilogue {
+    double eps;
+    int crop_h, crop_w;
+
+    __device__ __forceinline__ void begin(const Geo&, long long) {}
+    __device__ __forceinline__ EpiOut<A> operator()(A mux, A muy, A vx, A vy, A cxy, const Geo& g, long long oh,
+                                                    long long ow) const {
+        const A s = (((A)2 * (mux * muy)) * ((A)2 * cxy)) / ((mux * mux + muy * muy) * (vx + vy) + (A)eps);
+        const bool in_crop = crop_h > 0 && crop_w > 0 && oh >= crop_h && oh < g.oh - crop_h && ow >= crop_w &&
+                             ow < g.ow - crop_w;
+        return {s, in_crop ? (double)s : 0.0, 0.0};
+    }
+};
+
+// VIF-P, one scale (functional/image/vif.py:63-82): x is preds, y is target.  The reference's masks in its order, then
+// log10(1 + g²σt / (σv + σn²)) into s0 and log10(1 + σt / σn²) into s1.  No map.
+template <typename A>
+struct VifEpilogue {
+    double eps, sigma_n_sq;  // rounded to the input dtype by the caller, as torch.tensor(..., dtype=dtype) rounds them
+
+    __device__ __forceinline__ void begin(const Geo&, long long) {}
+    __device__ __forceinline__ EpiOut<A> operator()(A, A, A vx, A vy, A cxy, const Geo&, long long, long long) const {
+        const A e = (A)eps, sn = (A)sigma_n_sq;
+        A st = vy;
+        A gain = cxy / (st + e);
+        A sv = vx - gain * cxy;
+        if (st < e) {
+            gain = 0;
+            sv = vx;
+            st = 0;
+        }
+        if (vx < e) {
+            gain = 0;
+            sv = 0;
+        }
+        if (gain < (A)0) {
+            sv = vx;
+            gain = 0;
+        }
+        sv = sv < e ? e : sv;  // torch.clamp(min=eps): NaN stays NaN
+        return {(A)0, (double)log10((A)1 + gain * gain * st / (sv + sn)), (double)log10((A)1 + st / sn)};
+    }
+};
+
+// grid: one CTA per (image, channel, output depth, tile row, tile column), in that order, slowest first.  A CTA's slot
+// holds its two epilogue sums, so the slots of one image, and of one (image, channel), are consecutive.
+// Two CTAs per SM, as K20 has always run: without the bound, ptxas holds some epilogue instantiations to 80 registers
+// and spills.
+template <typename T, int TH, class Epi>
+__global__ void __launch_bounds__(kThreads, 2) ssim_kernel(Vol P, Vol Q, Geo g, const T* __restrict__ weights, Clamp cl,
+                                                        Epi epi, T* __restrict__ map, double2* __restrict__ partials) {
     using A = typename Cvt<T>::A;
     constexpr int RPT = TH / kWarps;  // output rows per thread
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -291,16 +381,9 @@ __global__ void __launch_bounds__(kThreads) ssim_kernel(Vol P, Vol Q, Geo g, con
             for (int j = 0; j < RPT; ++j) acc[m][j] += wd * v[m][j];
     }
 
-    A c1, c2;
-    if (consts) {
-        c1 = (A)consts[MB200_SSIM_C1];
-        c2 = (A)consts[MB200_SSIM_C2];
-    } else {
-        c1 = (A)c1_arg;
-        c2 = (A)c2_arg;
-    }
+    Epi e = epi;
+    e.begin(g, od);
     const A sx = shift[0], sy = shift[1];
-    const bool depth_in_crop = !g.crop_depth || (g.pd > 0 && od >= g.pd && od < g.od - g.pd);
     double ssum = 0.0, csum = 0.0;
     const long long ow = ow0 + lane;
 #pragma unroll
@@ -308,19 +391,14 @@ __global__ void __launch_bounds__(kThreads) ssim_kernel(Vol P, Vol Q, Geo g, con
         const long long oh = oh0 + rg * RPT + j;
         if (oh < g.oh && ow < g.ow) {
             const A mx = acc[0][j], my = acc[1][j];
-            const A mux = mx + sx, muy = my + sy;
             A vx = acc[2][j] - mx * mx;
             A vy = acc[3][j] - my * my;
             vx = vx < (A)0 ? (A)0 : vx;  // torch.clamp(min=0): NaN stays NaN
             vy = vy < (A)0 ? (A)0 : vy;
-            const A cxy = acc[4][j] - mx * my;
-            const A upper = (A)2 * cxy + c2;
-            const A lower = (vx + vy) + c2;
-            const A s = (((A)2 * (mux * muy) + c1) * upper) / ((mux * mux + muy * muy + c1) * lower);
-            ssum += (double)s;
-            if (map) map[(((bi * g.c + ch) * g.od + od) * g.oh + oh) * g.ow + ow] = Cvt<T>::from_a(s);
-            if (depth_in_crop && g.ph > 0 && g.pw > 0 && oh >= g.ph && oh < g.oh - g.ph && ow >= g.pw && ow < g.ow - g.pw)
-                csum += (double)(upper / lower);
+            const EpiOut<A> r = e(mx + sx, my + sy, vx, vy, acc[4][j] - mx * my, g, oh, ow);
+            ssum += r.s0;
+            csum += r.s1;
+            if (map) map[(((bi * g.c + ch) * g.od + od) * g.oh + oh) * g.ow + ow] = Cvt<T>::from_a(r.map);
         }
     }
     ssum = warp_sum(ssum);
@@ -475,6 +553,56 @@ __global__ void __launch_bounds__(kThreads) pool_kernel(Vol P, Vol Q, Geo g, int
     }
 }
 
+// ---- VIF decimation between scales --------------------------------------------------------------------------------------
+// conv2d(x, k)[..., ::2, ::2] of both inputs (functional/image/vif.py:49-51): the valid separable filter evaluated at even
+// output positions only, per depth plane, in the accumulation type, rounded to the preds dtype.  No shift: filtering is
+// linear, so nothing cancels.  Each axis's taps are divided by their float64 sum, as in ssim_kernel.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) decimate_kernel(Vol P, Vol Q, Geo g, const T* __restrict__ weights,
+                                                            T* __restrict__ po, T* __restrict__ qo) {
+    using A = typename Cvt<T>::A;
+    __shared__ A wt[2 * MB200_SSIM_MAX_TAPS];
+    const int kh = g.kh, kw = g.kw;
+    A* wH = wt;
+    A* wW = wt + kh;
+    for (int i = threadIdx.x; i < kh + kw; i += kThreads) wt[i] = Cvt<T>::to_a(weights[i]);
+    __syncthreads();
+    if (threadIdx.x < 2) {
+        A* w = threadIdx.x == 0 ? wH : wW;
+        const int k = threadIdx.x == 0 ? kh : kw;
+        double sum = 0.0;
+        for (int i = 0; i < k; ++i) sum += (double)w[i];
+        for (int i = 0; i < k; ++i) w[i] = (A)((double)w[i] / sum);
+    }
+    __syncthreads();
+    const Clamp none{0, 0.0, 0.0};
+    const long long n = g.b * g.c * g.d * g.oh * g.ow;
+    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kThreads) {
+        long long q = i;
+        const long long x = q % g.ow;
+        q /= g.ow;
+        const long long y = q % g.oh;
+        q /= g.oh;
+        const long long z = q % g.d;
+        q /= g.d;
+        const long long ci = q % g.c, bi = q / g.c;
+        const long long oP = bi * P.sn + ci * P.sc + z * P.sd + 2 * y * P.sh + 2 * x * P.sw;
+        const long long oQ = bi * Q.sn + ci * Q.sc + z * Q.sd + 2 * y * Q.sh + 2 * x * Q.sw;
+        A sp = 0, sq = 0;
+        for (int a = 0; a < kh; ++a) {
+            A rp = 0, rq = 0;
+            for (int c = 0; c < kw; ++c) {
+                rp += wW[c] * load_px<T>(P, oP + a * P.sh + c * P.sw, none);
+                rq += wW[c] * load_px<T>(Q, oQ + a * Q.sh + c * Q.sw, none);
+            }
+            sp += wH[a] * rp;
+            sq += wH[a] * rq;
+        }
+        po[i] = Cvt<T>::from_a(sp);
+        qo[i] = Cvt<T>::from_a(sq);
+    }
+}
+
 // ---- host side ----------------------------------------------------------------------------------------------------------
 struct Layout {
     long long od, oh, ow, tiles_h, tiles_w, tiles, smem;
@@ -503,6 +631,29 @@ Layout layout(long long b, long long c, long long d, long long h, long long w, i
 }
 
 long long align16(long long v) { return (v + 15) / 16 * 16; }
+
+Geo geo(const Layout& L, long long b, long long c, long long d, long long h, long long w, int kd, int kh, int kw, int pd,
+        int ph, int pw, int crop_depth) {
+    return Geo{b, c, d, h, w, kd, kh, kw, pd, ph, pw, L.od, L.oh, L.ow, crop_depth ? 1 : 0, L.tiles_h, L.tiles_w};
+}
+
+// the moment pass with epilogue `epi`, then one finalize CTA per group of consecutive slots (an image, or an (image,
+// channel)): s0[group] = its first sums / count, s1[group] = its second sums / count1 (s1 NULL: not written)
+template <typename T, class Epi>
+int moments(const Vol& P, const Vol& Q, const Layout& L, const Geo& g, const void* weights, const Clamp& cl, const Epi& epi,
+            void* map, void* scratch, long long groups, double count, double count1, double* s0, double* s1,
+            cudaStream_t st) {
+    constexpr int TH = Tile<T>::kH;
+    double2* partials = reinterpret_cast<double2*>(scratch);
+    MB200_CUDA_OK(ensure_dynamic_smem(ssim_kernel<T, TH, Epi>, kMaxSmem));
+    ssim_kernel<T, TH, Epi><<<(unsigned)L.tiles, kThreads, (size_t)L.smem, st>>>(
+        P, Q, g, reinterpret_cast<const T*>(weights), cl, epi, reinterpret_cast<T*>(map), partials);
+    count_launch();
+    finalize_kernel<<<(unsigned)groups, kThreads, 0, st>>>(partials, L.tiles / groups, count, count1, s0, s1);
+    count_launch();
+    MB200_CUDA_OK(cudaGetLastError());
+    return 0;
+}
 
 long long scratch_for(const Layout& L) { return align16(L.tiles * (long long)sizeof(double2)) + kRangeBlocks * 4 * 8; }
 
@@ -594,22 +745,13 @@ extern "C" int mb200_ssim_update(const void* preds, int preds_dtype, const void*
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     return with_float_type(preds_dtype, [&](auto tag) -> int {
         using T = typename decltype(tag)::type;
-        constexpr int TH = Tile<T>::kH;
+        using A = typename Cvt<T>::A;
         const Layout L = layout<T>(b, c, d, h, w, taps_d, taps_h, taps_w, pad_d, pad_h, pad_w);
-        Geo g{b, c, d, h, w, taps_d, taps_h, taps_w, pad_d, pad_h, pad_w, L.od, L.oh, L.ow, crop_depth ? 1 : 0, L.tiles_h,
-              L.tiles_w};
-        double2* partials = reinterpret_cast<double2*>(scratch);
-        MB200_CUDA_OK(ensure_dynamic_smem(ssim_kernel<T, TH>, kMaxSmem));
-        ssim_kernel<T, TH><<<(unsigned)L.tiles, kThreads, (size_t)L.smem, st>>>(
-            P, Q, g, reinterpret_cast<const T*>(weights), cl, consts, c1, c2, reinterpret_cast<T*>(map), partials);
-        count_launch();
         auto crop = [](long long o, int p) -> long long { return p > 0 ? std::max(0ll, o - 2ll * p) : 0ll; };
         const double crop_count = (double)c * (crop_depth ? crop(L.od, pad_d) : L.od) * crop(L.oh, pad_h) * crop(L.ow, pad_w);
-        finalize_kernel<<<(unsigned)b, kThreads, 0, st>>>(partials, L.tiles / b, (double)(c * L.od * L.oh * L.ow),
-                                                          crop_count, sim, cs);
-        count_launch();
-        MB200_CUDA_OK(cudaGetLastError());
-        return 0;
+        const SsimEpilogue<A> epi{consts, c1, c2, (A)0, (A)0, false};
+        return moments<T>(P, Q, L, geo(L, b, c, d, h, w, taps_d, taps_h, taps_w, pad_d, pad_h, pad_w, crop_depth), weights,
+                          cl, epi, map, scratch, b, (double)(c * L.od * L.oh * L.ow), crop_count, sim, cs, st);
     });
 }
 
@@ -636,5 +778,109 @@ extern "C" int mb200_ssim_avg_pool(const void* preds, int preds_dtype, const voi
         count_launch();
         MB200_CUDA_OK(cudaGetLastError());
         return 0;
+    });
+}
+
+#define MB200_MOMENT_CHECK_FILTER()                                                                                    \
+    MB200_REQUIRE(b >= 0 && c >= 1 && d >= 1 && h >= 1 && w >= 1, "bad sizes");                                      \
+    MB200_REQUIRE(taps_d >= 1 && taps_h >= 1 && taps_w >= 1 && taps_d <= MB200_SSIM_MAX_TAPS &&                      \
+                      taps_h <= MB200_SSIM_MAX_TAPS && taps_w <= MB200_SSIM_MAX_TAPS,                                \
+                  "tap counts must lie in [1, %d], got %d, %d, %d", MB200_SSIM_MAX_TAPS, taps_d, taps_h, taps_w)
+
+extern "C" int mb200_vif_scale_update(const void* preds, int preds_dtype, const void* target, int target_dtype,
+                                      int64_t b, int64_t c, int64_t d, int64_t h, int64_t w, int64_t preds_s_n,
+                                      int64_t preds_s_c, int64_t preds_s_d, int64_t preds_s_h, int64_t preds_s_w,
+                                      int64_t target_s_n, int64_t target_s_c, int64_t target_s_d, int64_t target_s_h,
+                                      int64_t target_s_w, int taps_d, int taps_h, int taps_w, const void* weights,
+                                      double eps, double sigma_n_sq, double* preds_sum, double* target_sum,
+                                      void* scratch, int64_t scratch_bytes, void* stream) {
+    MB200_SSIM_CHECK_TAGS();
+    MB200_MOMENT_CHECK_FILTER();
+    const int64_t need = mb200_ssim_scratch_bytes(preds_dtype, b, c, d, h, w, taps_d, taps_h, taps_w, 0, 0, 0);
+    MB200_REQUIRE(need >= 0,
+                  "the filter (%d, %d, %d taps) gives an empty output or does not fit in shared memory, or the batch has "
+                  "2^31 tiles or more", taps_d, taps_h, taps_w);
+    MB200_REQUIRE(preds && target && weights && preds_sum && target_sum && scratch, "NULL pointer");
+    MB200_REQUIRE(scratch_bytes >= need && (reinterpret_cast<uintptr_t>(scratch) & 15) == 0,
+                  "scratch must be 16-byte aligned and mb200_ssim_scratch_bytes(...) bytes");
+    if (b == 0) return 0;
+    const Vol P{preds, preds_dtype, preds_s_n, preds_s_c, preds_s_d, preds_s_h, preds_s_w};
+    const Vol Q{target, target_dtype, target_s_n, target_s_c, target_s_d, target_s_h, target_s_w};
+    const Clamp none{0, 0.0, 0.0};
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    return with_float_type(preds_dtype, [&](auto tag) -> int {
+        using T = typename decltype(tag)::type;
+        using A = typename Cvt<T>::A;
+        const Layout L = layout<T>(b, c, d, h, w, taps_d, taps_h, taps_w, 0, 0, 0);
+        const VifEpilogue<A> epi{eps, sigma_n_sq};
+        return moments<T>(P, Q, L, geo(L, b, c, d, h, w, taps_d, taps_h, taps_w, 0, 0, 0, 0), weights, none, epi, nullptr,
+                          scratch, b * c, 1.0, 1.0, preds_sum, target_sum, st);
+    });
+}
+
+extern "C" int mb200_vif_decimate(const void* preds, int preds_dtype, const void* target, int target_dtype, int64_t b,
+                                  int64_t c, int64_t d, int64_t h, int64_t w, int64_t preds_s_n, int64_t preds_s_c,
+                                  int64_t preds_s_d, int64_t preds_s_h, int64_t preds_s_w, int64_t target_s_n,
+                                  int64_t target_s_c, int64_t target_s_d, int64_t target_s_h, int64_t target_s_w,
+                                  int taps_h, int taps_w, const void* weights, void* preds_out, void* target_out,
+                                  void* stream) {
+    MB200_SSIM_CHECK_TAGS();
+    MB200_REQUIRE(b >= 0 && c >= 1 && d >= 1 && h >= 1 && w >= 1, "bad sizes");
+    MB200_REQUIRE(taps_h >= 1 && taps_w >= 1 && taps_h <= MB200_SSIM_MAX_TAPS && taps_w <= MB200_SSIM_MAX_TAPS,
+                  "tap counts must lie in [1, %d], got %d, %d", MB200_SSIM_MAX_TAPS, taps_h, taps_w);
+    MB200_REQUIRE(taps_h <= h && taps_w <= w, "the filter (%d, %d taps) gives an empty output on %lld x %lld", taps_h,
+                  taps_w, (long long)h, (long long)w);
+    MB200_REQUIRE(preds && target && weights && preds_out && target_out, "NULL pointer");
+    Geo g{};
+    g.b = b, g.c = c, g.d = d, g.h = h, g.w = w, g.kh = taps_h, g.kw = taps_w;
+    g.oh = (h - taps_h + 2) / 2;  // ceil((h - taps_h + 1) / 2): the even positions of the valid output
+    g.ow = (w - taps_w + 2) / 2;
+    const long long n = b * c * d * g.oh * g.ow;
+    if (n == 0) return 0;
+    const Vol P{preds, preds_dtype, preds_s_n, preds_s_c, preds_s_d, preds_s_h, preds_s_w};
+    const Vol Q{target, target_dtype, target_s_n, target_s_c, target_s_d, target_s_h, target_s_w};
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const unsigned blocks = (unsigned)std::min<long long>(cdiv(n, kThreads), 65536ll * 4);
+    return with_float_type(preds_dtype, [&](auto tag) -> int {
+        using T = typename decltype(tag)::type;
+        decimate_kernel<T><<<blocks, kThreads, 0, st>>>(P, Q, g, reinterpret_cast<const T*>(weights),
+                                                        reinterpret_cast<T*>(preds_out), reinterpret_cast<T*>(target_out));
+        count_launch();
+        MB200_CUDA_OK(cudaGetLastError());
+        return 0;
+    });
+}
+
+extern "C" int mb200_uqi_update(const void* preds, int preds_dtype, const void* target, int target_dtype, int64_t b,
+                                int64_t c, int64_t d, int64_t h, int64_t w, int64_t preds_s_n, int64_t preds_s_c,
+                                int64_t preds_s_d, int64_t preds_s_h, int64_t preds_s_w, int64_t target_s_n,
+                                int64_t target_s_c, int64_t target_s_d, int64_t target_s_h, int64_t target_s_w, int taps_d,
+                                int taps_h, int taps_w, int pad_d, int pad_h, int pad_w, int crop_h, int crop_w,
+                                const void* weights, double eps, double* sums, void* map, void* scratch,
+                                int64_t scratch_bytes, void* stream) {
+    MB200_SSIM_CHECK_TAGS();
+    MB200_MOMENT_CHECK_FILTER();
+    MB200_REQUIRE(pad_d >= 0 && pad_h >= 0 && pad_w >= 0 && pad_d < d && pad_h < h && pad_w < w,
+                  "reflect pads (%d, %d, %d) must be non-negative and below the sizes", pad_d, pad_h, pad_w);
+    MB200_REQUIRE(crop_h >= 0 && crop_w >= 0, "crop margins (%d, %d) must be non-negative", crop_h, crop_w);
+    const int64_t need = mb200_ssim_scratch_bytes(preds_dtype, b, c, d, h, w, taps_d, taps_h, taps_w, pad_d, pad_h, pad_w);
+    MB200_REQUIRE(need >= 0,
+                  "the filter (%d, %d, %d taps) gives an empty output or does not fit in shared memory, or the batch has "
+                  "2^31 tiles or more", taps_d, taps_h, taps_w);
+    MB200_REQUIRE(preds && target && weights && sums && scratch, "NULL pointer");
+    MB200_REQUIRE(scratch_bytes >= need && (reinterpret_cast<uintptr_t>(scratch) & 15) == 0,
+                  "scratch must be 16-byte aligned and mb200_ssim_scratch_bytes(...) bytes");
+    if (b == 0) return 0;
+    const Vol P{preds, preds_dtype, preds_s_n, preds_s_c, preds_s_d, preds_s_h, preds_s_w};
+    const Vol Q{target, target_dtype, target_s_n, target_s_c, target_s_d, target_s_h, target_s_w};
+    const Clamp none{0, 0.0, 0.0};
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    return with_float_type(preds_dtype, [&](auto tag) -> int {
+        using T = typename decltype(tag)::type;
+        using A = typename Cvt<T>::A;
+        const Layout L = layout<T>(b, c, d, h, w, taps_d, taps_h, taps_w, pad_d, pad_h, pad_w);
+        const UqiEpilogue<A> epi{eps, crop_h, crop_w};
+        return moments<T>(P, Q, L, geo(L, b, c, d, h, w, taps_d, taps_h, taps_w, pad_d, pad_h, pad_w, 0), weights, none,
+                          epi, map, scratch, b, 1.0, 1.0, sums, nullptr, st);
     });
 }

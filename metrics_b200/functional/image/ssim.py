@@ -40,10 +40,10 @@ def _ssim_check_inputs(preds: Tensor, target: Tensor) -> tuple[Tensor, Tensor]:
     return preds, target
 
 
-def _no_graph(preds: Tensor, target: Tensor) -> None:
+def _no_graph(preds: Tensor, target: Tensor, message: str = _NO_GRAPH) -> None:
     """The reference would build an autograd graph here; a kernel cannot, so say so instead of returning a constant."""
     if torch.is_grad_enabled() and (preds.requires_grad or target.requires_grad):
-        raise RuntimeError(_NO_GRAPH)
+        raise RuntimeError(message)
 
 
 def _filter_args(ndim: int, gaussian_kernel: bool, sigma, kernel_size, return_full_image: bool = False,
