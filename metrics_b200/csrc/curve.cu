@@ -47,13 +47,43 @@ __device__ __forceinline__ __nv_bfloat16 from_float<__nv_bfloat16>(float x) { re
 
 // ascending sort of this key == descending sort of the score; NaN first (torch.argsort(descending=True) puts NaN first)
 __device__ __forceinline__ unsigned desc_key(float v) { return ~f32_order_key(v); }
+
+// Runs the reference splits.  It finds thresholds with where(preds[1:] - preds[:-1]): NaN - NaN and inf - inf are NaN, so
+// every NaN, +inf or -inf score ends its own group.  Their desc keys sit at the two ends of the key range, next to the
+// NaN payloads no score maps to: NaN 0, +inf 0x007fffff, -inf 0xff800000 (64-bit: 0, 0x000fffffffffffff,
+// 0xfff0000000000000).  Inside such a run the order is fixed as negatives before positives, on every path: the bit-0 path
+// gets it from the label in the low bit, the pair paths from label_key, which moves one label of each special value to the
+// unused neighbour key (NaN 0/1, +inf 0x..fe/0x..ff, -inf 0x..00/0x..01 as (negative, positive)).
+template <typename KeyT>
+struct SpecialKeys {
+    static constexpr KeyT kPosInf = sizeof(KeyT) == 4 ? (KeyT)0x007fffffu : (KeyT)0x000fffffffffffffull;
+    static constexpr KeyT kNegInf = sizeof(KeyT) == 4 ? (KeyT)0xff800000u : (KeyT)0xfff0000000000000ull;
+};
+// true for the keys of NaN, +inf and -inf (and their label neighbours): k < kPosInf + 1 or k >= kNegInf, as one compare
+template <typename KeyT>
+__device__ __forceinline__ bool is_special_key(KeyT k) {
+    return (KeyT)(k + (SpecialKeys<KeyT>::kPosInf + 1)) < (KeyT)(2 * (SpecialKeys<KeyT>::kPosInf + 1));
+}
+template <typename KeyT>
+__device__ __forceinline__ KeyT label_key(KeyT k, bool positive) {
+    if (positive) return (k == 0 || k == SpecialKeys<KeyT>::kNegInf) ? k + 1 : k;
+    return k == SpecialKeys<KeyT>::kPosInf ? k - 1 : k;
+}
+// the canonical key of a label_key result
+template <typename KeyT>
+__device__ __forceinline__ KeyT canonical_key(KeyT k) {
+    if (k == 1) return 0;
+    if (k == SpecialKeys<KeyT>::kPosInf - 1) return SpecialKeys<KeyT>::kPosInf;
+    if (k == SpecialKeys<KeyT>::kNegInf + 1) return SpecialKeys<KeyT>::kNegInf;
+    return k;
+}
 __device__ __forceinline__ float score_of_key(unsigned k) {
-    const unsigned ok = ~k;
+    const unsigned ok = ~canonical_key(k);
     if (ok == 0xffffffffu) return __int_as_float(0x7fc00000);
     return f32_from_order_key(ok);
 }
 __device__ __forceinline__ double score_of_key(unsigned long long k) {
-    const unsigned long long ok = ~k;
+    const unsigned long long ok = ~canonical_key(k);
     if (ok == ~0ull) return __longlong_as_double(0x7ff8000000000000ll);
     const unsigned long long b = (ok & 0x8000000000000000ull) ? (ok & 0x7fffffffffffffffull) : ~ok;
     return __longlong_as_double((long long)b);
@@ -414,7 +444,7 @@ __global__ void __launch_bounds__(256) pack_binary_kernel(const T* __restrict__ 
 #pragma unroll
                 for (int p = 0; p < 4; ++p) atomicAdd(&sh_hist[p * 256 + ((ck >> (8 * p)) & 255u)], 1u);
             } else {
-                keys[i] = k;
+                keys[i] = label_key(k, one != 0u);
                 labels[i] = (unsigned char)one;
             }
         }
@@ -437,12 +467,12 @@ __global__ void __launch_bounds__(256) pack_ovr_kernel(const T* __restrict__ pre
                                                        typename KeyOf<T>::type* __restrict__ keys,
                                                        unsigned char* __restrict__ labels, unsigned* __restrict__ err = nullptr) {
     __shared__ typename KeyOf<T>::type tile[32][33];
-    __shared__ int tgt[32];
+    __shared__ long long tgt[32];  // compared in 64 bits: an int64 target of 2^32 + c is not class c
     const int n0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;  // 8 rows of 32 threads
     if (threadIdx.x < 32) {
         const int nn = n0 + threadIdx.x;
-        tgt[threadIdx.x] = nn < n ? (int)load_label(target, tdtype, nn) : -1;
+        tgt[threadIdx.x] = nn < n ? load_label(target, tdtype, nn) : -1;
     }
     for (int j = ty; j < 32; j += 8) {
         const int nn = n0 + j, cc = c0 + tx;
@@ -458,8 +488,9 @@ __global__ void __launch_bounds__(256) pack_ovr_kernel(const T* __restrict__ pre
                 keys[(size_t)cc * n + nn] = (k << 1) | (typename KeyOf<T>::type)(tgt[tx] == cc);
                 continue;
             }
-            keys[(size_t)cc * n + nn] = tile[tx][j];
-            labels[(size_t)cc * n + nn] = (unsigned char)(tgt[tx] == cc);
+            const bool one = tgt[tx] == cc;
+            keys[(size_t)cc * n + nn] = label_key(tile[tx][j], one);
+            labels[(size_t)cc * n + nn] = (unsigned char)one;
         }
     }
 }
@@ -485,8 +516,9 @@ __global__ void __launch_bounds__(256) pack_multilabel_kernel(const T* __restric
         if (nn < n && cc < L) {
             const long long t = load_label(target, tdtype, (long long)nn * L + cc);
             const bool ign = has_ignore && t == ignore;
-            tile[j][tx] = ign ? kIgnoredKey : KeyOf<T>::make(preds[(size_t)nn * L + cc]);
-            ltile[j][tx] = (unsigned char)(t == 1 && !ign);
+            const bool one = t == 1 && !ign;
+            tile[j][tx] = ign ? kIgnoredKey : label_key(KeyOf<T>::make(preds[(size_t)nn * L + cc]), one);
+            ltile[j][tx] = (unsigned char)one;
         }
     }
     __syncthreads();
@@ -523,15 +555,18 @@ __global__ void __launch_bounds__(256) pack_keys_kernel(const T* __restrict__ pr
     }
 }
 
-// labels[s][i] = (target[i] == first_class + s)
-__global__ void __launch_bounds__(256) labels_from_target_kernel(const void* __restrict__ target, int tdtype, int n,
-                                                                 int segments, long long first_class,
+// labels[s][i] = (target[i] == first_class + s); the keys of NaN / +-inf scores move to their label's key (label_key)
+__global__ void __launch_bounds__(256) labels_from_target_kernel(unsigned* __restrict__ keys, const void* __restrict__ target,
+                                                                 int tdtype, int n, int segments, long long first_class,
                                                                  unsigned char* __restrict__ labels) {
     const long long total = (long long)n * segments;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int s = (int)(i / n);
         const int k = (int)(i - (long long)s * n);
-        labels[i] = (unsigned char)(load_label(target, tdtype, k) == first_class + s);
+        const bool one = load_label(target, tdtype, k) == first_class + s;
+        labels[i] = (unsigned char)one;
+        const unsigned key = keys[i];
+        if (is_special_key(key)) keys[i] = label_key(key, one);
     }
 }
 
@@ -771,7 +806,7 @@ __global__ void __launch_bounds__(kChainThreads, sizeof(KeyT) == 4 ? 4 : 2) scan
         bool e = false;
         if (i < count) {
             const KeyT nk = (i + 1 < kChainItems) ? key[i + 1] : key_next;
-            e = (base + i == n - 1) || key[i] != nk;
+            e = (base + i == n - 1) || key[i] != nk || is_special_key(key[i]);  // NaN / +-inf: one group each
         }
         if (e) {
             ends |= 1u << i;
@@ -927,11 +962,12 @@ __global__ void __launch_bounds__(kChainThreads, sizeof(KeyT) == 4 ? 4 : 2) scan
 // A private-API path of the reference (no public functional passes weights): built for exactness, not for speed.
 // =====================================================================================================
 template <typename T>
-__global__ void __launch_bounds__(256) pack_indexed_kernel(const T* __restrict__ preds, long long n,
+__global__ void __launch_bounds__(256) pack_indexed_kernel(const T* __restrict__ preds, const void* __restrict__ target,
+                                                           int tdtype, long long pos_label, long long n,
                                                            typename KeyOf<T>::type* __restrict__ keys,
                                                            unsigned* __restrict__ idx) {
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-        keys[i] = KeyOf<T>::make(preds[i]);
+        keys[i] = label_key(KeyOf<T>::make(preds[i]), load_label(target, tdtype, i) == pos_label);
         idx[i] = (unsigned)i;
     }
 }
@@ -965,7 +1001,7 @@ __global__ void __launch_bounds__(kWThreads) weighted_curve_kernel(const KeyT* _
             const bool pos = load_label(target, tdtype, src) == pos_label;
             wp = pos ? w : 0.0;
             wn = pos ? 0.0 : w;
-            end = (i == n - 1 || keys[i + 1] != k) ? 1u : 0u;
+            end = (i == n - 1 || keys[i + 1] != k || is_special_key(k)) ? 1u : 0u;
         }
         // inclusive block scans of (wp, wn, end) in a fixed order
         double ip = wp, in_ = wn;
@@ -1220,7 +1256,8 @@ int evaluate_multilabel_typed(const void* preds, const void* target, int target_
     if (has_ignore) MB200_CUDA_OK(cudaMemsetAsync(w.seg_ignored, 0, (size_t)num_labels * sizeof(int), st));
     const dim3 grid((unsigned)((ni + 31) / 32), (unsigned)((num_labels + 31) / 32));
     pack_multilabel_kernel<T><<<grid, 256, 0, st>>>(reinterpret_cast<const T*>(preds), target, target_dtype, ni, (int)num_labels,
-                                                    has_ignore, (long long)ignore_index, w.keys_a, w.lab_a, w.seg_ignored);
+                                                    has_ignore, label_ignore_index(ignore_index, target_dtype), w.keys_a,
+                                                    w.lab_a, w.seg_ignored);
     count_launch();
     return sort_and_scan<KeyT>(w.keys_a, w.lab_a, w, ni, num_labels, n, has_ignore ? w.seg_ignored : nullptr, out_auroc, out_ap,
                                out_counts, fps_out, tps_out, thr_out, err_flag, st);
@@ -1336,7 +1373,7 @@ extern "C" int mb200_curve_evaluate_keys(uint32_t* keys, const void* target, int
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     CurveWs<unsigned> w = carve<unsigned>(workspace, segments, n);
     const long long total = n * segments;
-    labels_from_target_kernel<<<blocks_for(total, 256 * 8, sm_count() * 8), 256, 0, st>>>(target, target_dtype, (int)n,
+    labels_from_target_kernel<<<blocks_for(total, 256 * 8, sm_count() * 8), 256, 0, st>>>(keys, target, target_dtype, (int)n,
                                                                                           (int)segments, first_class, w.lab_a);
     count_launch();
     return sort_and_scan<unsigned>(keys, w.lab_a, w, (int)n, segments, n, nullptr, out_auroc, out_ap, out_counts, nullptr, nullptr,
@@ -1374,7 +1411,8 @@ int weighted_typed(const void* preds, const void* target, int target_dtype, cons
     unsigned* idx_a = (unsigned*)bump(p, n * 4);
     unsigned* idx_b = (unsigned*)bump(p, n * 4);
     unsigned* scratch = (unsigned*)bump(p, (int64_t)radix_sort_scratch_words(n, 1, (int)sizeof(KeyT)) * 4);
-    pack_indexed_kernel<T><<<blocks_for(n, 256 * 4, sm_count() * 8), 256, 0, st>>>(reinterpret_cast<const T*>(preds), n, keys_a,
+    pack_indexed_kernel<T><<<blocks_for(n, 256 * 4, sm_count() * 8), 256, 0, st>>>(reinterpret_cast<const T*>(preds), target,
+                                                                                  target_dtype, (long long)pos_label, n, keys_a,
                                                                                   idx_a);
     count_launch();
     const int where = radix_sort_passes<KeyT, unsigned>(keys_a, idx_a, keys_b, idx_b, (int)n, 1, (int)sizeof(KeyT), scratch,

@@ -38,10 +38,16 @@ def binary_clf_curve(preds: np.ndarray, target: np.ndarray, pos_label: int = 1, 
     """_binary_clf_curve (functional/classification/precision_recall_curve.py:30-82).
     Returns integer fps, tps (int64) and thresholds (preds dtype), thresholds descending; with `sample_weights` (:64, :73-78)
     fps / tps are float64 weighted cumulative sums.  float64 scores are compared as float64 (no down-cast anywhere)."""
-    order = np.argsort(-preds.astype(np.float64), kind="stable")  # :60 argsort(descending=True)
+    # :60 argsort(descending=True), NaN first like torch; inside runs of NaN, +inf or -inf (which :70 splits into one threshold
+    # per element) the order the kernels fix: negatives before positives
+    p64 = preds.astype(np.float64)
+    nan = np.isnan(p64)
+    second = np.where(~np.isfinite(p64), (target == pos_label).astype(np.int64), 0)
+    order = np.lexsort((second, -np.where(nan, 0.0, p64), ~nan))
     p = preds[order]
     t = (target[order] == pos_label).astype(np.int64)  # :72
-    distinct = np.nonzero(p[1:] - p[:-1])[0]  # :70
+    with np.errstate(invalid="ignore"):
+        distinct = np.nonzero(p[1:] - p[:-1])[0]  # :70 (NaN - NaN, inf - inf: NaN, nonzero)
     idx = np.concatenate([distinct, [t.size - 1]])  # :71
     if sample_weights is not None:
         w = np.asarray(sample_weights, dtype=np.float64)[order]  # :64
