@@ -82,6 +82,7 @@ def lib() -> ctypes.CDLL:
 # time of a small `update()` — and makes a wrong argument count or kind a TypeError instead of a silent truncation.
 _C_TYPES = {"i": ctypes.c_int, "q": ctypes.c_int64, "Q": ctypes.c_uint64, "d": ctypes.c_double, "p": ctypes.c_void_p,
             "s": ctypes.c_char_p}
+_VOL = "pipi" + "q" * 15  # image kernels: preds, its tag, target, its tag, [b, c, d, h, w], preds strides, target strides
 SIGNATURES = {
     # include/metrics_b200.h
     "mb200_abi_version": ("i", ""),
@@ -158,13 +159,7 @@ SIGNATURES = {
     # include/metrics_b200_hausdorff.h
     "mb200_hausdorff_scratch_bytes": ("q", "qqiq"),
     "mb200_hausdorff_distance": ("i", "pipiiqqqqqqqqqqqqiiiddiqppqpp"),
-}
-
-
-# include/mb200_image.h (K20, K21), outside the include/metrics_b200*.h set until it joins the one drive table of
-# tests/test_abi.py; tests/test_image_abi.py checks it
-_VOL = "pipi" + "q" * 15  # preds, its tag, target, its tag, [b, c, d, h, w], preds strides, target strides
-IMAGE_SIGNATURES = {
+    # include/metrics_b200_image.h
     "mb200_ssim_scratch_bytes": ("q", "iqqqqqiiiiii"),
     "mb200_ssim_data_range": ("i", _VOL + "ddppqp"),
     "mb200_ssim_update": ("i", _VOL + "iiiiiiipiddpddppppqp"),
@@ -177,7 +172,7 @@ IMAGE_SIGNATURES = {
 
 def declare_signatures(handle) -> None:
     """Set ``restype`` / ``argtypes`` of every exported function on a loaded library handle."""
-    for name, (ret, args) in {**SIGNATURES, **IMAGE_SIGNATURES}.items():
+    for name, (ret, args) in SIGNATURES.items():
         fn = getattr(handle, name)
         fn.restype = _C_TYPES[ret]
         fn.argtypes = [_C_TYPES[a] for a in args]
@@ -1424,7 +1419,7 @@ def hausdorff_distance(preds: Tensor, target: Tensor, num_classes: int, index_fo
 
 
 # ----------------------------------------------------------------------------------------------------------
-# K20 wrappers (structural similarity, include/mb200_image.h)
+# K20 wrappers (structural similarity, include/metrics_b200_image.h)
 # ----------------------------------------------------------------------------------------------------------
 SSIM_RANGE, SSIM_C1, SSIM_C2, SSIM_CONSTS = 0, 1, 2, 3
 SSIM_MAX_TAPS = 255
@@ -1438,9 +1433,14 @@ def _volume(x: Tensor) -> tuple[tuple, tuple]:
     return tuple(x.shape), tuple(x.stride())
 
 
-def ssim_scratch_bytes(preds: Tensor, taps: tuple, pads: tuple) -> int:
-    shape, _ = _volume(preds)
-    return int(lib().mb200_ssim_scratch_bytes(tag(preds), *shape, *taps, *pads))
+def _moment_scratch(preds: Tensor, shape: tuple, taps: tuple, pads: tuple, dev) -> tuple[Tensor, int]:
+    """The scratch of one windowed-moment pass (K20, K21) and its size in bytes."""
+    nbytes = int(lib().mb200_ssim_scratch_bytes(tag(preds), *shape, *taps, *pads))
+    if nbytes < 0:
+        raise ValueError(f"metrics_b200: a filter of {tuple(taps)} taps with pads {tuple(pads)} on {tuple(shape[2:])} "
+                         f"needs more than one CTA's shared memory or gives an empty output, or the batch of {shape[0]} x "
+                         f"{shape[1]} planes needs 2^31 tiles or more")
+    return torch.empty(nbytes, dtype=torch.uint8, device=dev), nbytes
 
 
 def ssim(preds: Tensor, target: Tensor, weights: Tensor, taps: tuple, pads: tuple, crop_depth: bool,
@@ -1456,12 +1456,7 @@ def ssim(preds: Tensor, target: Tensor, weights: Tensor, taps: tuple, pads: tupl
     _, ts = _volume(target)
     b = shape[0]
     lib_ = lib()
-    nbytes = int(lib_.mb200_ssim_scratch_bytes(tag(preds), *shape, *taps, *pads))
-    if nbytes < 0:
-        raise ValueError(f"metrics_b200: a filter of {tuple(taps)} taps with pads {tuple(pads)} on {tuple(shape[2:])} "
-                         f"needs more than one CTA's shared memory or gives an empty output, or the batch of {shape[0]} x "
-                         f"{shape[1]} planes needs 2^31 tiles or more")
-    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    scratch, nbytes = _moment_scratch(preds, shape, taps, pads, dev)
     sim = torch.empty(b, dtype=torch.float64, device=dev)
     cs = torch.empty(b, dtype=torch.float64, device=dev) if want_cs else None
     out_shape = (shape[0], shape[1], *(n + 2 * p - k + 1 for n, p, k in zip(shape[2:], pads, taps)))
@@ -1508,17 +1503,8 @@ def ssim_avg_pool(preds: Tensor, target: Tensor, pool_depth: bool) -> tuple[Tens
 
 
 # ----------------------------------------------------------------------------------------------------------
-# K21 wrappers (VIF and UQI on K20's moments, include/mb200_image.h)
+# K21 wrappers (VIF and UQI on K20's moments, include/metrics_b200_image.h)
 # ----------------------------------------------------------------------------------------------------------
-def _moment_scratch(preds: Tensor, shape: tuple, taps: tuple, pads: tuple, dev) -> tuple[Tensor, int]:
-    nbytes = int(lib().mb200_ssim_scratch_bytes(tag(preds), *shape, *taps, *pads))
-    if nbytes < 0:
-        raise ValueError(f"metrics_b200: a filter of {tuple(taps)} taps with pads {tuple(pads)} on {tuple(shape[2:])} "
-                         f"needs more than one CTA's shared memory or gives an empty output, or the batch of {shape[0]} x "
-                         f"{shape[1]} planes needs 2^31 tiles or more")
-    return torch.empty(nbytes, dtype=torch.uint8, device=dev), nbytes
-
-
 def vif_scale(preds: Tensor, target: Tensor, weights: Tensor, taps: tuple, eps: float,
               sigma_n_sq: float) -> tuple[Tensor, Tensor]:
     """K21, one VIF scale with valid filtering: float64 ``[b, c]`` sums of the preds term and of the target term.

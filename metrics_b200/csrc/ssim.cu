@@ -22,7 +22,7 @@
 #include <algorithm>
 
 #include "common.cuh"
-#include "../../include/mb200_image.h"
+#include "../../include/metrics_b200_image.h"
 
 namespace mb200 {
 

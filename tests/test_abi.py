@@ -21,7 +21,7 @@ STREAM = 0xABCD
 
 
 def _source(path):
-    """The header without its comments."""
+    """A header or CUDA source without its comments."""
     text = re.sub(r"/\*.*?\*/", "", open(path).read(), flags=re.S)
     return re.sub(r"//[^\n]*", "", text)
 
@@ -54,6 +54,16 @@ def test_signature_table_matches_the_headers():
     assert _native.SIGNATURES == declared
 
 
+def test_every_header_and_export_is_in_the_one_table():
+    """A header the glob misses, or an entry point the library defines but no header declares, would bind outside
+    `_native.SIGNATURES` and escape every check here."""
+    assert sorted(glob.glob(os.path.join(ROOT, "include", "*.h"))) == HEADERS
+    defined = set()
+    for path in glob.glob(os.path.join(ROOT, "metrics_b200", "csrc", "*.cu")):
+        defined.update(re.findall(r'extern\s+"C"\s+[\w\s\*]+?\b(mb200_\w+)\s*\(', _source(path)))
+    assert defined == set(_native.SIGNATURES)
+
+
 def test_library_exports_every_declared_symbol():
     assert os.path.exists(_native.lib_path()), "build the extension first: python -c 'import __graft_entry__ as g; g.build()'"
     raw = ctypes.CDLL(_native.lib_path())
@@ -75,7 +85,8 @@ def test_header_constants_match_the_binding():
     mirrors = ("ABI_VERSION F32 F16 BF16 F64 I64 I32 I16 I8 U8 BOOL FLAG_TARGET_RANGE FLAG_PREDS_RANGE FLAG_SPIN_TIMEOUT "
                "FLAG_CAPACITY SEG_PREDS_NEGATIVE SEG_PREDS_TOO_LARGE SEG_TARGET_NEGATIVE SEG_TARGET_TOO_LARGE RET_AP RET_RR "
                "RET_PRECISION RET_RECALL RET_HIT_RATE RET_FALL_OUT RET_R_PRECISION RET_NDCG RET_MAX_ELEMENTS RANKCORR_MAX_ROWS "
-               "PQ_UNKNOWN_PREDS HD_PREDS_NOT_BINARY HD_TARGET_NOT_BINARY HD_NO_EDGES").split()
+               "PQ_UNKNOWN_PREDS HD_PREDS_NOT_BINARY HD_TARGET_NOT_BINARY HD_NO_EDGES SSIM_RANGE SSIM_C1 SSIM_C2 SSIM_CONSTS "
+               "SSIM_MAX_TAPS").split()
     assert {k: getattr(_native, k) for k in mirrors} == {k: header[k] for k in mirrors}
     assert _native.KENDALL_VARIANT == {v: header["KENDALL_" + v.upper()] for v in "abc"}
     assert _native.KENDALL_ALTERNATIVE == {a: header["KENDALL_ALT_" + (a or "none").upper().replace("-", "_")]
@@ -160,6 +171,15 @@ def _drives():
     cl = oh.to(torch.uint8)
     strided = torch.rand(6, 4, 5, 6)[::2]
     groups = _native.RetrievalGroups(i64(n), torch.rand(n), i64(n + 1), i64(2), 1, 0)
+    # K20 and K21 read channels-last preds and a transposed target through their strides
+    ssim_preds = torch.zeros(2, 3, 20, 24).contiguous(memory_format=torch.channels_last)
+    ssim_target = torch.zeros(2, 3, 24, 20, dtype=torch.float64).transpose(2, 3)
+    vif_preds = torch.zeros(2, 3, 41, 45).contiguous(memory_format=torch.channels_last)
+    vif_target = torch.zeros(2, 3, 45, 41).transpose(2, 3)
+
+    def ssim(data_range=None, clamp=None):
+        return _native.ssim(ssim_preds, ssim_target, torch.ones(23), (1, 11, 11), (0, 5, 5), False, clamp, data_range, 0.01,
+                            0.03, True, True)
 
     def hausdorff_one_hot():
         # a cap of four of the recorder's 1000-byte pairs, so that the 9 pairs do not fit one launch
@@ -252,16 +272,23 @@ def _drives():
         "hausdorff_one_hot": hausdorff_one_hot,
         "hausdorff_index": lambda: _native.hausdorff_distance(i64(2, 9, 6).transpose(1, 2), i64(2, 9, 6).transpose(1, 2), 5, True,
                                                               False, "euclidean", [1, 1], False),
+        # K20: structural similarity; K21: VIF and UQI
+        "ssim": ssim,
+        "ssim_fixed_range_clamp": lambda: ssim(0.5, (0.25, 0.75)),
+        "ssim_avg_pool": lambda: _native.ssim_avg_pool(torch.zeros(2, 3, 9, 10, 11), torch.zeros(2, 3, 9, 10, 11).half(), True),
+        "vif_scale": lambda: _native.vif_scale(vif_preds, vif_target, torch.ones(40), (1, 17, 17), 1e-10, 2.0),
+        "vif_decimate": lambda: _native.vif_decimate(vif_preds, vif_target, torch.ones(40), (9, 9)),
+        "uqi": lambda: _native.uqi(vif_preds, vif_target, torch.ones(40), (1, 11, 5), (0, 2, 5), (5, 2), 1e-7, True),
     }
 
 
 DRIVES = _drives()
 
 
-def test_every_kernel_wrapper_calls_the_abi_as_declared(monkeypatch):
+def test_every_drive_calls_the_abi_as_declared(monkeypatch):
     """Run every drive once (CPU tensors, device checks patched out, library replaced by `_Recorder`): argument count and C
     types must match the headers, pointers must be non-NULL where a tensor was passed, and the stream handle must arrive as
-    the last argument."""
+    the last argument.  Every entry point of `_native.SIGNATURES` that is not a C-only query must be called by some drive."""
     real = _native.lib()
     seg_sizes = {(fmt, dt): real.mb200_segmentation_scratch_bytes(4, 19, 4096, fmt, 1, dt, 0)
                  for fmt in (0, 1) for dt in (_native.F16, _native.BOOL)}
@@ -282,7 +309,7 @@ def test_every_kernel_wrapper_calls_the_abi_as_declared(monkeypatch):
 
     # (`mb200_regression_num_sums` is a query for C callers; the Python mirror knows the layout of each op's sums)
     kernels = {k for k in _native.SIGNATURES if k not in ("mb200_abi_version", "mb200_last_error", "mb200_regression_num_sums",
-                                                          "mb200_curve_workspace_bytes", "mb200_binary_stat_counts")}
+                                                          "mb200_binary_stat_counts")}
     never_called = sorted(kernels - {name for calls in fake.calls.values() for name in calls})
     assert not never_called, f"no wrapper exercised: {never_called}"
     for drive, calls in fake.calls.items():
@@ -359,6 +386,41 @@ def test_every_kernel_wrapper_calls_the_abi_as_declared(monkeypatch):
     assert all(v not in (None, 0) for v in (hd[0], hd[2], hd[24], hd[25], hd[27]))
     index = call("hausdorff_index", "mb200_hausdorff_distance")  # index labels pass three strides
     assert index[4:9] == (0, 2, 5, 6, 9) and index[9:13] == (54, 0, 1, 6) and index[19] == 3 and index[23] == 10
+
+    sim, cs, img = results["ssim"]
+    assert sim.shape == cs.shape == (2,) and sim.dtype == torch.float64 and img.shape == (2, 3, 1, 20, 24)
+    rng, upd = call("ssim", "mb200_ssim_data_range"), call("ssim", "mb200_ssim_update")
+    for v in (rng, upd):  # float32 channels-last preds, float64 transposed target
+        assert v[1] == _native.F32 and v[3] == _native.F64 and v[4:9] == (2, 3, 1, 20, 24)
+        assert v[9:14] == (1440, 1, 0, 72, 3) and v[14:19] == (1440, 480, 0, 1, 20)
+    assert rng[19:21] == (0.01, 0.03) and rng[22] is not None and rng[-2] == 256  # the scratch the library asked for
+    assert upd[19:26] == (1, 11, 11, 0, 5, 5, 0) and upd[27] == 0  # taps, pads, no depth crop, no clamp
+    assert upd[30] == rng[21] and all(upd[k] is not None for k in (26, 33, 34, 35, 36))  # consts of the pre-pass
+    assert upd[33:36] == (sim.data_ptr(), cs.data_ptr(), img.data_ptr())
+    assert "mb200_ssim_data_range" not in fake.calls["ssim_fixed_range_clamp"]
+    fixed = call("ssim_fixed_range_clamp", "mb200_ssim_update")
+    assert fixed[27:33] == (1, 0.25, 0.75, None, (0.01 * 0.5) ** 2, (0.03 * 0.5) ** 2)
+    po, to = results["ssim_avg_pool"]
+    assert po.shape == to.shape == (2, 3, 4, 5, 5) and to.dtype == torch.float32
+    pool = call("ssim_avg_pool", "mb200_ssim_avg_pool")
+    assert pool[3] == _native.F16 and pool[4:9] == (2, 3, 9, 10, 11) and pool[19] == 1
+    assert pool[20:22] == (po.data_ptr(), to.data_ptr())
+
+    preds_sum, target_sum = results["vif_scale"]
+    assert preds_sum.shape == target_sum.shape == (2, 3) and preds_sum.dtype == torch.float64
+    po, to = results["vif_decimate"]
+    assert po.shape == to.shape == (2, 3, 17, 19) and po.dtype == torch.float32  # ceil((41 - 9 + 1) / 2), (45 - 9 + 2) // 2
+    sums, img = results["uqi"]
+    assert sums.shape == (2,) and img.shape == (2, 3, 1, 41 + 4 - 11 + 1, 45 + 10 - 5 + 1)
+    vs, dc, uq = call("vif_scale", "mb200_vif_scale_update"), call("vif_decimate", "mb200_vif_decimate"), call("uqi", "mb200_uqi_update")
+    for v in (vs, dc, uq):  # float32 channels-last preds, float32 transposed target
+        assert v[1] == v[3] == _native.F32 and v[4:9] == (2, 3, 1, 41, 45)
+        assert v[9:14] == (5535, 1, 0, 135, 3) and v[14:19] == (5535, 1845, 0, 1, 41)
+    assert vs[19:22] == (1, 17, 17) and vs[23:25] == (1e-10, 2.0) and vs[-2] == 256
+    assert vs[25:27] == (preds_sum.data_ptr(), target_sum.data_ptr())
+    assert dc[19:21] == (9, 9) and all(v is not None for v in dc[21:24]) and dc[22:24] == (po.data_ptr(), to.data_ptr())
+    assert uq[19:27] == (1, 11, 5, 0, 2, 5, 5, 2) and uq[28] == 1e-7 and uq[30] is not None and uq[-2] == 256
+    assert uq[29:31] == (sums.data_ptr(), img.data_ptr())
 
 
 def test_real_library_accepts_every_wrappers_arguments_up_to_the_first_cuda_call(monkeypatch):

@@ -139,6 +139,27 @@ ENTRIES = {
     "hausdorff_index": ({I64}, INVALID, "index labels must be int64 (dtype tags %d, 4)", lambda L, b, d: _hausdorff(L, b, d, 0)),
 }
 
+# K20 and K21 on one 16 x 16 (SSIM) or 48 x 48 (VIF, UQI) image: call(lib, buffers, preds tag, target tag)
+SSIM_GEO = (1, 1, 1, 16, 16) + (256, 256, 0, 16, 1) * 2
+VIF_GEO = (1, 1, 1, 48, 48) + (2304, 2304, 0, 48, 1) * 2
+_IMAGE = {
+    "ssim_update": lambda L, b, dp, dt: L.mb200_ssim_update(b.p, dp, b.t, dt, *SSIM_GEO, 1, 3, 3, 0, 1, 1, 0, b.weights, 0, 0.0, 0.0,
+                                                            None, 1.0, 1.0, b.out, None, None, b.ws, NBYTES, 0),
+    "ssim_data_range": lambda L, b, dp, dt: L.mb200_ssim_data_range(b.p, dp, b.t, dt, *SSIM_GEO, 0.01, 0.03, b.acc, b.ws, NBYTES, 0),
+    "ssim_avg_pool": lambda L, b, dp, dt: L.mb200_ssim_avg_pool(b.p, dp, b.t, dt, *SSIM_GEO, 0, b.out, b.acc, 0),
+    "vif_scale_update": lambda L, b, dp, dt: L.mb200_vif_scale_update(b.p, dp, b.t, dt, *VIF_GEO, 1, 17, 17, b.weights, 1e-10, 2.0,
+                                                                      b.fps, b.tps, b.ws, NBYTES, 0),
+    "vif_decimate": lambda L, b, dp, dt: L.mb200_vif_decimate(b.p, dp, b.t, dt, *VIF_GEO, 9, 9, b.weights, b.out, b.acc, 0),
+    "uqi_update": lambda L, b, dp, dt: L.mb200_uqi_update(b.p, dp, b.t, dt, *VIF_GEO, 1, 11, 11, 0, 5, 5, 5, 5, b.weights, 1e-7,
+                                                          b.out, None, b.ws, NBYTES, 0),
+}
+for _name, _call in _IMAGE.items():
+    # the preds tag varied with a float32 target, then the target tag with float32 preds
+    ENTRIES[_name] = (FLOAT, INVALID, "preds must be a floating-point tensor (dtype tag %d)",
+                      lambda L, b, d, _call=_call: _call(L, b, d, F32))
+    ENTRIES[_name + "_target"] = (FLOAT, INVALID, "target must be a floating-point tensor (dtype tag %d)",
+                                  lambda L, b, d, _call=_call: _call(L, b, F32, d))
+
 
 @pytest.mark.parametrize("name", sorted(ENTRIES))
 def test_rejected_tags_fail_before_any_cuda_work(name):

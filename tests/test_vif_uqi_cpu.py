@@ -1,8 +1,8 @@
 """CPU: VIF and UQI (kernel K21).  The float64 oracles (oracle/vif.py, oracle/uqi.py) and the reference's torch chains
 against the goldens made from the unmodified reference (tests/golden/vif_uqi.npz); the public surface, state registries
 and error paths against tests/golden/vif_uqi_surface.json; every golden replayed through the classes and functionals
-with the oracles standing in for the kernels; and the C-ABI of the three new entry points."""
-import ctypes
+with the oracles standing in for the kernels.  The C-ABI of K21 is checked in tests/test_abi.py,
+tests/test_dtype_dispatch_abi.py and tests/test_image_abi.py."""
 import json
 import os
 import warnings
@@ -17,7 +17,6 @@ from oracle import vif as ovf
 from tests import vif_uqi_cases as vc
 from tests.conftest import GOLDEN_DIR
 from tests.golden.make_golden_vif_uqi import error_calls, modules, states, surface
-from tests.test_abi import _patch_host
 
 CASES = vc.cases()
 IDS = [c["name"] for c in CASES]
@@ -139,98 +138,3 @@ def test_goldens_through_classes_and_functionals_on_the_standin(host, case):
         if case["dtype"] == "f64":
             assert np.allclose(value, want, rtol=0, atol=_tol(case), equal_nan=True), (key, value, want)
 
-
-# ---- C-ABI ------------------------------------------------------------------------------------------------------------
-STREAM = 0xCAFE
-NEW = ("mb200_vif_scale_update", "mb200_vif_decimate", "mb200_uqi_update")
-
-
-class _Recorder:
-    def __init__(self):
-        self.calls = {}
-        for name, (ret, args) in _native.IMAGE_SIGNATURES.items():
-            def callback(*values, _name=name):
-                self.calls.setdefault(_name, []).append(values)
-                return 4096 if _name.endswith("_bytes") else 0
-
-            setattr(self, name, ctypes.CFUNCTYPE(_native._C_TYPES[ret], *[_native._C_TYPES[a] for a in args])(callback))
-
-
-def _drives():
-    p = torch.zeros(2, 3, 41, 45).contiguous(memory_format=torch.channels_last)
-    t = torch.zeros(2, 3, 45, 41).transpose(2, 3)
-    w = torch.ones(40)
-    return p, t, w, (
-        lambda: _native.vif_scale(p, t, w, (1, 17, 17), 1e-10, 2.0),
-        lambda: _native.vif_decimate(p, t, w, (9, 9)),
-        lambda: _native.uqi(p, t, w, (1, 11, 5), (0, 2, 5), (5, 2), 1e-7, True),
-    )
-
-
-def test_new_wrappers_call_the_abi_as_declared(monkeypatch):
-    fake = _Recorder()
-    monkeypatch.setattr(_native, "lib", lambda: fake)
-    _patch_host(monkeypatch, STREAM)
-    p, t, w, (scale, decimate, uqi) = _drives()
-    a, b = scale()
-    assert a.shape == b.shape == (2, 3) and a.dtype == torch.float64
-    po, to = decimate()
-    assert po.shape == to.shape == (2, 3, 17, 19) and po.dtype == torch.float32  # ceil((41 - 9 + 1) / 2), (45 - 9 + 2) // 2
-    sums, img = uqi()
-    assert sums.shape == (2,) and img.shape == (2, 3, 1, 41 + 4 - 11 + 1, 45 + 10 - 5 + 1)
-    for name in NEW:
-        (call,) = fake.calls[name]
-        assert len(call) == len(_native.IMAGE_SIGNATURES[name][1]) and call[-1] == STREAM
-        assert call[1] == _native.F32 and call[3] == _native.F32 and call[4:9] == (2, 3, 1, 41, 45)
-        assert call[9:14] == (p.stride(0), p.stride(1), 0, p.stride(2), p.stride(3))
-        assert call[14:19] == (t.stride(0), t.stride(1), 0, t.stride(2), t.stride(3))
-    vs, dc, uq = (fake.calls[n][0] for n in NEW)
-    assert vs[19:22] == (1, 17, 17) and vs[23:25] == (1e-10, 2.0) and vs[-2] == 4096
-    assert dc[19:21] == (9, 9) and all(v is not None for v in dc[21:24])
-    assert uq[19:27] == (1, 11, 5, 0, 2, 5, 5, 2) and uq[28] == 1e-7 and uq[30] is not None and uq[-2] == 4096
-
-
-def test_real_library_accepts_the_new_wrappers_arguments_up_to_the_first_cuda_call(monkeypatch):
-    if torch.cuda.is_available():
-        pytest.skip("a CUDA device is present: host pointers must not reach the kernels")
-    _patch_host(monkeypatch, 0)
-    for drive in _drives()[3]:
-        with pytest.raises(_native.NativeLibraryError, match=r"\(code -2\): CUDA error"):
-            drive()
-
-
-@pytest.mark.parametrize("bad", [-1, _native.I64, _native.I32, _native.U8, _native.BOOL, 10])
-def test_new_entry_points_reject_non_float_dtype_tags_before_any_launch(bad):
-    lib = _native.lib()
-    geo = (1, 1, 1, 48, 48) + (2304, 2304, 0, 48, 1) * 2
-    for which, msg in ((0, f"preds must be a floating-point tensor (dtype tag {bad})"),
-                       (1, f"target must be a floating-point tensor (dtype tag {bad})")):
-        tags = (bad, _native.F32) if which == 0 else (_native.F32, bad)
-        for rc in (lib.mb200_vif_scale_update(8, tags[0], 8, tags[1], *geo, 1, 17, 17, 8, 1e-10, 2.0, 8, 8, 16, 1 << 20,
-                                              None),
-                   lib.mb200_vif_decimate(8, tags[0], 8, tags[1], *geo, 9, 9, 8, 8, 8, None),
-                   lib.mb200_uqi_update(8, tags[0], 8, tags[1], *geo, 1, 11, 11, 0, 5, 5, 5, 5, 8, 1e-7, 8, None, 16,
-                                        1 << 20, None)):
-            assert rc == -1 and lib.mb200_last_error().decode() == msg
-
-
-def test_new_entry_points_reject_bad_geometry_before_any_launch():
-    lib = _native.lib()
-    geo = (1, 1, 1, 48, 48) + (2304, 2304, 0, 48, 1) * 2
-    small = (1, 1, 1, 16, 16) + (256, 256, 0, 16, 1) * 2
-    f = _native.F32
-    checks = [
-        (lambda: lib.mb200_vif_scale_update(8, f, 8, f, *geo, 1, 0, 17, 8, 1e-10, 2.0, 8, 8, 16, 1 << 20, None), "tap counts"),
-        (lambda: lib.mb200_vif_scale_update(8, f, 8, f, *geo, 1, 256, 17, 8, 1e-10, 2.0, 8, 8, 16, 1 << 20, None), "tap counts"),
-        (lambda: lib.mb200_vif_scale_update(8, f, 8, f, *small, 1, 17, 17, 8, 1e-10, 2.0, 8, 8, 16, 1 << 20, None), "empty output"),
-        (lambda: lib.mb200_vif_decimate(8, f, 8, f, *small, 17, 9, 8, 8, 8, None), "empty output"),
-        (lambda: lib.mb200_vif_decimate(8, f, 8, f, *geo, 0, 9, 8, 8, 8, None), "tap counts"),
-        (lambda: lib.mb200_uqi_update(8, f, 8, f, *small, 1, 11, 11, 0, 16, 5, 5, 5, 8, 1e-7, 8, None, 16, 1 << 20, None),
-         "reflect pads"),
-        (lambda: lib.mb200_uqi_update(8, f, 8, f, *small, 1, 11, 11, 0, 5, 5, -1, 5, 8, 1e-7, 8, None, 16, 1 << 20, None),
-         "crop margins"),
-        (lambda: lib.mb200_uqi_update(8, f, 8, f, *small, 1, 41, 11, 0, 5, 5, 5, 5, 8, 1e-7, 8, None, 16, 1 << 20, None),
-         "empty output"),
-    ]
-    for call, msg in checks:
-        assert call() == -1 and msg in lib.mb200_last_error().decode(), msg
