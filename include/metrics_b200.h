@@ -141,14 +141,15 @@ MB200_API int mb200_curve_sigmoid_if_logits(const void* preds, int dtype, int64_
                                             uint32_t* flag_scratch, void* stream);
 /* softmax(dim=1) variant for [n, num_classes] row-major scores (multiclass curve metrics,
  * functional/classification/precision_recall_curve.py:454). */
-/* mb200_curve_softmax_if_logits with a caller-owned scratch of 8 + n bytes (4-byte aligned, contents irrelevant): rows of at
+/* mb200_curve_softmax_if_logits with a caller-owned scratch of 8 + n bytes (4-byte aligned, contents irrelevant; a shorter or
+ * unaligned scratch takes the original kernels with its first aligned word as the vote word): rows of at
  * most 1024 f32 / f16 / bf16 scores are read ONCE (row kept in registers, one `expf` per score); a row that itself holds a score
  * outside [0, 1] writes its softmax, the others are written through and revisited by a second (normally empty) launch only when
  * the batch turned out to be logits.  Same bits as mb200_curve_softmax_if_logits. */
 MB200_API int mb200_curve_softmax_if_logits_scratch(const void* preds, int dtype, int64_t n, int64_t num_classes, void* out,
                                                     void* scratch, int64_t scratch_bytes, void* stream);
 /* mb200_curve_sigmoid_if_logits with a caller-owned scratch of mb200_curve_normalize_scratch_bytes(n) bytes (4-byte aligned,
- * contents irrelevant): large 16-byte aligned f32 / f16 / bf16 batches are then read ONCE — every 16 KB tile that itself
+ * contents irrelevant; an unaligned scratch takes the original kernels with its first aligned word as the vote word): large 16-byte aligned f32 / f16 / bf16 batches are then read ONCE — every 16 KB tile that itself
  * holds a score outside [0, 1] knows the vote and writes sigmoids, the others write the scores through and are revisited by a
  * second (normally empty) launch only when the batch turned out to be logits. */
 MB200_API int64_t mb200_curve_normalize_scratch_bytes(int64_t n);

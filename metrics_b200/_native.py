@@ -408,7 +408,20 @@ def sigmoid_if_logits(preds: Tensor) -> Tensor:
 
 
 def softmax_if_logits(preds: Tensor) -> Tensor:
-    """``normalize_logits_if_needed(preds, "softmax")`` for a contiguous ``[N, C]`` tensor."""
+    """``normalize_logits_if_needed(preds, "softmax")``: softmax over dim 1 of an ``[N, C, ...]`` tensor when any score of the
+    batch lies outside [0, 1] (the reference's ``torch.softmax(tensor, dim=1)``).  Extra dims are folded into ``[M, C]`` rows
+    with the class dim last and unfolded afterwards; the vote stays batch-wide over every element."""
+    if preds.ndim < 2:
+        raise ValueError(f"softmax normalisation expects an [N, C, ...] tensor, got {preds.ndim} dimension(s)")
+    if preds.ndim > 2:
+        moved = preds.movedim(1, -1)
+        rows = _softmax_rows(moved.reshape(-1, preds.shape[1]))
+        return rows.reshape(moved.shape).movedim(-1, 1).contiguous()
+    return _softmax_rows(preds)
+
+
+def _softmax_rows(preds: Tensor) -> Tensor:
+    """`softmax_if_logits` of ``[N, C]`` rows."""
     if _TORCH_BINDING:
         return _ops().normalize_logits_if_needed(preds, "softmax")
     dev = require_cuda(preds)

@@ -1456,6 +1456,13 @@ extern "C" int64_t mb200_curve_normalize_scratch_bytes(int64_t n) {
     return 8 + (n / 1024 + 2);  // vote word + one byte per 16 KB tile (tiles hold >= 1024 elements)
 }
 
+// The vote word of the original kernels inside a caller-owned scratch: its first 4-byte aligned word (the word is the
+// target of atomicOr, which needs natural alignment), or NULL (an error) when the scratch holds no such word.
+static uint32_t* vote_word(void* scratch, int64_t scratch_bytes) {
+    const uintptr_t a = (reinterpret_cast<uintptr_t>(scratch) + 3) & ~uintptr_t(3);
+    return (int64_t)(a - reinterpret_cast<uintptr_t>(scratch)) + 4 <= scratch_bytes ? reinterpret_cast<uint32_t*>(a) : nullptr;
+}
+
 // mb200_curve_sigmoid_if_logits with a caller-owned scratch of mb200_curve_normalize_scratch_bytes(n): large aligned
 // f32 / f16 / bf16 batches then take the speculative single pass (one read + one write); everything else the original path.
 extern "C" int mb200_curve_sigmoid_if_logits_scratch(const void* preds, int dtype, int64_t n, void* out, void* scratch,
@@ -1467,7 +1474,7 @@ extern "C" int mb200_curve_sigmoid_if_logits_scratch(const void* preds, int dtyp
     const bool spec = dtype != MB200_F64 && n > 1024 * kSmallItems &&
                       ((reinterpret_cast<uintptr_t>(preds) | reinterpret_cast<uintptr_t>(out)) & 15) == 0 &&
                       (reinterpret_cast<uintptr_t>(scratch) & 3) == 0;
-    if (!spec) return mb200_curve_sigmoid_if_logits(preds, dtype, n, out, reinterpret_cast<uint32_t*>(scratch), stream);
+    if (!spec) return mb200_curve_sigmoid_if_logits(preds, dtype, n, out, vote_word(scratch, scratch_bytes), stream);
     MB200_REQUIRE(is_float_tag<kNoF64>(dtype), "scores must be floating point (dtype tag %d)", dtype);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int esize = dtype == MB200_F32 ? 4 : 2;
@@ -1503,7 +1510,7 @@ extern "C" int mb200_curve_softmax_if_logits_scratch(const void* preds, int dtyp
     MB200_REQUIRE(n < (1ll << 31) && num_classes < (1ll << 31), "sizes exceed int32");
     const bool spec = dtype != MB200_F64 && num_classes <= 1024 && scratch_bytes >= 8 + n &&
                       (reinterpret_cast<uintptr_t>(scratch) & 3) == 0;
-    if (!spec) return mb200_curve_softmax_if_logits(preds, dtype, n, num_classes, out, reinterpret_cast<uint32_t*>(scratch), stream);
+    if (!spec) return mb200_curve_softmax_if_logits(preds, dtype, n, num_classes, out, vote_word(scratch, scratch_bytes), stream);
     MB200_REQUIRE(is_float_tag<kNoF64>(dtype), "softmax scores must be f32/f16/bf16/f64 (dtype tag %d)", dtype);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     MB200_CUDA_OK(cudaMemsetAsync(scratch, 0, (size_t)(8 + n), st));
