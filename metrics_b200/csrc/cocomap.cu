@@ -5,11 +5,11 @@
 // `pycocotools.cocoeval.COCOeval` (`evaluate` / `accumulate`; `summarize` stays in Python here too) and `maskApi.c:bbIou`.
 // The algorithm restated (and cited step by step) in oracle/coco_map.py is what these kernels implement:
 //
-//   evaluate   one CTA per image: class index lookup, per-(image, class) score ranks (stable, = mergesort on -score),
-//              greedy matching for every (class, area range, IoU threshold) with fp64 IoUs computed on the fly from the
-//              fp32 xywh boxes, crowd / area-range ignore rules, per-detection match+ignore bit words (area*T + thr),
+//   evaluate   one CTA per image: class index lookup, per-(image, class) score ranks (stable, = mergesort on -score,
+//              NaN last), greedy matching for every (class, area range, IoU threshold) with fp64 IoUs computed on the
+//              fly from the fp32 xywh boxes, crowd / area-range ignore rules, per-detection match+ignore bit words (area*T + thr),
 //              non-ignored ground-truth counts per (class, area).
-//   sort       stable LSD radix sort of all detections by (class, score desc) — 64-bit key, 32-bit payload
+//   sort       stable LSD radix sort of all detections by (class, score desc, NaN last) — 64-bit key, 32-bit payload
 //              (radix_sort.cuh); the natural order (image, original index) is exactly COCOeval's concatenation order.
 //   accumulate one CTA per (class, area, maxDet): compaction to rank < maxDet, integer TP/FP prefix sums per IoU
 //              threshold, fp64 precision with `np.spacing(1)`, right-to-left running maximum, 101-point
@@ -97,12 +97,20 @@ __device__ __forceinline__ double mask_iou(double inter, double det_area, double
     return inter / (crowd ? det_area : det_area + gt_area - inter);
 }
 
+// COCOeval's detection order (`np.argsort(-score, kind="mergesort")`, per image in evaluateImg and across images in
+// accumulate) as an ascending u32 key: descending score, -0 and +0 equal, NaN after everything (-inf included); equal keys keep
+// the input order.  The per-image rank and the accumulate sort key both use it.  (f32_order_key puts NaN on top, as
+// torch.argmax does; negated, that would sort NaN first.)
+__device__ __forceinline__ unsigned coco_det_order_key(float s) {
+    return s != s ? 0xffffffffu : ~f32_order_key(s);
+}
+
 __host__ __device__ inline size_t map_eval_smem_bytes(int max_d, int max_g) {
     size_t b = 0;
     b += (size_t)(max_d + max_g) * 8;       // mask areas (mask mode; boxes leave them unused)
     b += (size_t)max_d * (16 + 8 + 8);      // box, match word, ignore word
     b += (size_t)max_g * (16 + 8);          // box, area
-    b += (size_t)max_d * (4 + 4 + 4 + 4);   // score, cat, rank, by_pos
+    b += (size_t)max_d * (4 + 4 + 4 + 4);   // score key, cat, rank, by_pos
     b += (size_t)max_g * (4 + 4);           // cat, crowd(int)
     b += (size_t)(max_d + max_g) * 4 * 3;   // cats list, cat_start, cat_cnt
     return b + 64;
@@ -126,7 +134,7 @@ __global__ void __launch_bounds__(256) map_evaluate_kernel(MapEvalArgs p, int ma
     double* gmarea = reinterpret_cast<double*>(ptr); ptr += (size_t)max_g * 8;  //            ground-truth mask areas
     const bool masks = p.pair_inter != nullptr;
     const double* __restrict__ inter_tab = masks ? p.pair_inter + p.pair_off[img] : nullptr;
-    float* dscore = reinterpret_cast<float*>(ptr); ptr += (size_t)max_d * 4;
+    unsigned* dkey = reinterpret_cast<unsigned*>(ptr); ptr += (size_t)max_d * 4;  // coco_det_order_key of the score
     int* dcat = reinterpret_cast<int*>(ptr); ptr += (size_t)max_d * 4;
     int* drank = reinterpret_cast<int*>(ptr); ptr += (size_t)max_d * 4;
     int* by_pos = reinterpret_cast<int*>(ptr); ptr += (size_t)max_d * 4;
@@ -143,7 +151,7 @@ __global__ void __launch_bounds__(256) map_evaluate_kernel(MapEvalArgs p, int ma
     if (tid == 0) ncats = 0;
     for (int i = tid; i < D; i += nth) {
         dbox[i] = p.det_box[d0 + i];
-        dscore[i] = p.det_score[d0 + i];
+        dkey[i] = coco_det_order_key(p.det_score[d0 + i]);
         dcat[i] = p.micro ? 0 : class_index(p.classes, p.K, p.det_label[d0 + i]);
         dmatch[i] = 0ull;
         dign[i] = 0ull;
@@ -160,13 +168,13 @@ __global__ void __launch_bounds__(256) map_evaluate_kernel(MapEvalArgs p, int ma
     }
     __syncthreads();
 
-    // ---- per-(image, class) rank by descending score, ties by original index (== mergesort on -score) ----
+    // ---- per-(image, class) rank in COCOeval's order (coco_det_order_key, ties by original index) ----
     for (int i = tid; i < D; i += nth) {
         const int c = dcat[i];
-        const float s = dscore[i];
+        const unsigned key = dkey[i];
         int r = 0;
         for (int j = 0; j < D; ++j)
-            if (dcat[j] == c && (dscore[j] > s || (dscore[j] == s && j < i))) r++;
+            if (dcat[j] == c && (dkey[j] < key || (dkey[j] == key && j < i))) r++;
         drank[i] = r;
     }
     // ---- distinct classes of this image (detections and ground truths) ----
@@ -272,14 +280,14 @@ __global__ void __launch_bounds__(256) map_evaluate_kernel(MapEvalArgs p, int ma
     }
 }
 
-// sort key: (class << 32) | inverted order key of the score; payload: detection index
+// sort key: (class << 32) | COCOeval order key of the score; payload: detection index
 __global__ void __launch_bounds__(256) map_pack_keys_kernel(const int* __restrict__ det_cat,
                                                             const float* __restrict__ det_score, int n,
                                                             unsigned long long* __restrict__ keys,
                                                             unsigned* __restrict__ vals) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) {
-        keys[i] = ((unsigned long long)(unsigned)det_cat[i] << 32) | (unsigned long long)(~f32_order_key(det_score[i]));
+        keys[i] = ((unsigned long long)(unsigned)det_cat[i] << 32) | (unsigned long long)coco_det_order_key(det_score[i]);
         vals[i] = (unsigned)i;
     }
 }

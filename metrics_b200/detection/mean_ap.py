@@ -62,8 +62,9 @@ def _pairwise_ious(det_box: Tensor, det_score: Tensor, det_label: Tensor, det_co
         table = torch.tensor(classes, dtype=torch.int64, device=dev)
         det_key = img_of_det * n_cls + torch.searchsorted(table, det_label)
         gt_key = img_of_gt * n_cls + torch.searchsorted(table, gt_label)
-    # detections: by (pair, score descending, input order); ground truths: by (pair, input order)
-    by_score = torch.sort(det_score, descending=True, stable=True).indices
+    # detections: by (pair, score descending, input order) in COCOeval's order (`argsort(-score, kind="mergesort")`): an
+    # ascending sort of `0 - score` puts NaN last and turns -0.0 into +0.0, so that +-0 tie; ground truths: by (pair, input order)
+    by_score = torch.sort(0.0 - det_score, stable=True).indices
     det_order = by_score[torch.sort(det_key[by_score], stable=True).indices]
     gt_order = torch.sort(gt_key, stable=True).indices
     n_pairs = n_img * n_cls

@@ -51,7 +51,25 @@ def box_convert_to_xywh(boxes: np.ndarray, fmt: str) -> np.ndarray:
 
 
 def bb_iou(dt: np.ndarray, gt: np.ndarray, iscrowd: np.ndarray) -> np.ndarray:
-    """maskApi.c:bbIou — IoU of xywh boxes in double; for a crowd gt the union is the detection's area."""
+    """maskApi.c:bbIou — IoU of xywh boxes in double; for a crowd gt the union is the detection's area.  Vectorised over the
+    [D, G] grid in bbIou's operation order: `np.fmin` / `np.fmax` are C's `fmin` / `fmax`, and numpy ufuncs never contract a
+    product and a sum into one FMA, so every value is the one the scalar loop (`bb_iou_scalar`) computes."""
+    d = dt.astype(np.float64).reshape(-1, 4)
+    g = gt.astype(np.float64).reshape(-1, 4)
+    dx, dy, dw, dh = (d[:, i:i + 1] for i in range(4))
+    gx, gy, gw, gh = (g[None, :, i] for i in range(4))
+    w = np.fmin(dx + dw, gx + gw) - np.fmax(dx, gx)
+    h = np.fmin(dy + dh, gy + gh) - np.fmax(dy, gy)
+    inter = w * h
+    da, ga = dw * dh, gw * gh
+    union = np.where(np.asarray(iscrowd, bool).reshape(1, -1), da, da + ga - inter)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        iou = inter / union
+    return np.where((w <= 0) | (h <= 0), 0.0, iou)  # `if (w <= 0) continue`: a NaN width is not skipped
+
+
+def bb_iou_scalar(dt: np.ndarray, gt: np.ndarray, iscrowd: np.ndarray) -> np.ndarray:
+    """bb_iou as maskApi.c:bbIou's loop, pair by pair (the check on the vectorised version; NaN-free boxes only)."""
     d = dt.astype(np.float64)
     g = gt.astype(np.float64)
     out = np.zeros((d.shape[0], g.shape[0]), dtype=np.float64)
@@ -316,3 +334,112 @@ def coco_evaluate(
     out["classes"] = classes.astype(np.int32)
     out["precision"], out["recall"], out["scores"] = precision, recall, scores
     return out
+
+
+# ---- the two phases of the device evaluation, as the records they exchange ----------------------------------------------
+# The kernels (csrc/cocomap.cu) split COCOeval into a per-image MATCH phase that writes one record per detection and an
+# ACCUMULATE phase that reads only those records (the sharded evaluation exchanges them between ranks).  These two functions
+# restate COCOeval in that shape; `accumulate_records(*match_records(...))` is `coco_evaluate`'s precision / recall / scores.
+
+
+def match_records(det_box, det_score, det_label, det_counts, gt_box, gt_label, gt_crowd, gt_area, gt_counts, classes,
+                  iou_thresholds, max_det_last, micro=False, pair_inter=None, pair_off=None, det_mask_area=None,
+                  gt_mask_area=None, gt_area_exact=False):
+    """COCOeval.evaluateImg for every (image, class, area range) of the given images, written out per detection: class index
+    (position of the label in the sorted `classes`; 0 for everything when `micro`), rank inside its (image, class) in
+    COCOeval's order (`np.argsort(-score, kind="mergesort")`: descending, NaN last, +-0 equal, ties by input position), and
+    uint64 match / ignore words with bit `area * T + threshold`; `npig` int32 [K, 4] counts the non-ignored ground truths.
+
+    Flat inputs: xywh float32 boxes, float32 scores, int64 labels, per-image counts; `gt_area` is the given area (<= 0 or -0.0:
+    w * h) unless `gt_area_exact`.  Mask mode (`pair_inter` not None): per image a flat [D, G] table of intersection pixel
+    counts at `pair_off[image]`, IoU = maskApi.c:rleIou from it and the mask areas, a detection's area range from its mask
+    area.  Only the first `max_det_last` detections of a (image, class) are matched; every detection gets a rank."""
+    thr = np.asarray(iou_thresholds, np.float64)
+    T = len(thr)
+    cls = np.asarray(classes, np.int64).reshape(-1)
+    K = 1 if micro else len(cls)
+    det_counts, gt_counts = [int(x) for x in det_counts], [int(x) for x in gt_counts]
+    n_det = sum(det_counts)
+    cat = np.zeros(n_det, np.int32)
+    rank = np.zeros(n_det, np.int32)
+    match = np.zeros(n_det, np.uint64)
+    ignore = np.zeros(n_det, np.uint64)
+    npig = np.zeros((K, 4), np.int32)
+    dbox = np.asarray(det_box, np.float32).reshape(-1, 4)
+    gbox = np.asarray(gt_box, np.float32).reshape(-1, 4)
+    dscore = np.asarray(det_score, np.float32).reshape(-1)
+    dlab, glab = np.asarray(det_label, np.int64).reshape(-1), np.asarray(gt_label, np.int64).reshape(-1)
+    gcrowd = np.asarray(gt_crowd).reshape(-1) != 0
+    given = np.asarray(gt_area, np.float64).reshape(-1)
+    gt_wh = gbox[:, 2].astype(np.float64) * gbox[:, 3].astype(np.float64)
+    garea = given if gt_area_exact else np.where(given > 0, given, gt_wh)
+    masks = pair_inter is not None
+    d0 = g0 = 0
+    for img, (nd, ng) in enumerate(zip(det_counts, gt_counts)):
+        dcat = np.zeros(nd, np.int64) if micro else np.searchsorted(cls, dlab[d0:d0 + nd])
+        gcat = np.zeros(ng, np.int64) if micro else np.searchsorted(cls, glab[g0:g0 + ng])
+        cat[d0:d0 + nd] = dcat
+        if masks:
+            table = np.asarray(pair_inter, np.float64)[int(pair_off[img]): int(pair_off[img]) + nd * ng].reshape(nd, ng)
+        for c in np.unique(np.concatenate([dcat, gcat])):
+            di, gi = np.flatnonzero(dcat == c), np.flatnonzero(gcat == c)
+            order = di[np.argsort(-dscore[d0 + di], kind="mergesort")]
+            rank[d0 + order] = np.arange(len(order))
+            top = order[:max_det_last]
+            for a, (lo, hi) in enumerate(AREA_RANGES):
+                g_ig = gcrowd[g0 + gi] | (garea[g0 + gi] < lo) | (garea[g0 + gi] > hi)
+                npig[c, a] += int((~g_ig).sum())
+                g_order = gi[np.argsort(g_ig, kind="mergesort")]
+                crowd_sorted = gcrowd[g0 + g_order]
+                if masks:
+                    inter = table[np.ix_(top, g_order)]
+                    da = np.asarray(det_mask_area, np.float64)[d0 + top][:, None]
+                    ga = np.asarray(gt_mask_area, np.float64)[g0 + g_order][None, :]
+                    with np.errstate(divide="ignore", invalid="ignore"):
+                        ious = np.where(inter > 0, inter / np.where(crowd_sorted[None, :], da, da + ga - inter), 0.0)
+                    d_area = np.asarray(det_mask_area, np.float64)[d0 + top]
+                else:
+                    ious = bb_iou(dbox[d0 + top], gbox[g0 + g_order], crowd_sorted)
+                    d_area = dbox[d0 + top, 2].astype(np.float64) * dbox[d0 + top, 3].astype(np.float64)
+                dtm, dt_ig = match_detections(ious, crowd_sorted, g_ig[np.argsort(g_ig, kind="mergesort")], thr)
+                dt_ig = dt_ig | ((dtm == 0) & ((d_area < lo) | (d_area > hi))[None, :])
+                for t in range(T):
+                    bit = np.uint64(1) << np.uint64(a * T + t)
+                    match[d0 + top[dtm[t] > 0]] |= bit
+                    ignore[d0 + top[dt_ig[t]]] |= bit
+        d0, g0 = d0 + nd, g0 + ng
+    return cat, rank, match, ignore, npig
+
+
+def accumulate_records(det_cat, det_score, det_rank, det_match, det_ignore, npig, num_classes, class_lo, class_hi, n_iou_thr,
+                       rec_thresholds, max_dets):
+    """COCOeval.accumulate from the per-detection records for the classes [class_lo, class_hi): per (class, area, maxDet) the
+    records of the class with rank < maxDet in COCOeval's score order (ties keep the order the records are given in), TP / FP
+    running sums, `sample_pr_curve`.  Full-size float64 `precision [T,R,K,4,M]`, `recall [T,K,4,M]`, `scores`, -1 outside the
+    range and where `npig == 0`."""
+    T, R, K, M = int(n_iou_thr), len(rec_thresholds), int(num_classes), len(max_dets)
+    rec = np.asarray(rec_thresholds, np.float64)
+    precision, recall, scores = -np.ones((T, R, K, 4, M)), -np.ones((T, K, 4, M)), -np.ones((T, R, K, 4, M))
+    cat, rank = np.asarray(det_cat).reshape(-1), np.asarray(det_rank).reshape(-1)
+    score = np.asarray(det_score, np.float32).reshape(-1).astype(np.float64)
+    match = np.asarray(det_match).reshape(-1).view(np.uint64)
+    ignore = np.asarray(det_ignore).reshape(-1).view(np.uint64)
+    n_valid = np.asarray(npig).reshape(-1, 4)
+    by_class = np.argsort(cat, kind="stable")
+    start = np.searchsorted(cat[by_class], np.arange(K + 1))
+    for k in range(int(class_lo), int(class_hi)):
+        in_class = by_class[start[k]:start[k + 1]]  # input order
+        for a in range(4):
+            if n_valid[k, a] == 0:
+                continue
+            for m, max_det in enumerate(max_dets):
+                sel = in_class[rank[in_class] < max_det]
+                sel = sel[np.argsort(-score[sel], kind="mergesort")]
+                for t in range(T):
+                    bit = np.uint64(1) << np.uint64(a * T + t)
+                    hit, ign = (match[sel] & bit) != 0, (ignore[sel] & bit) != 0
+                    tp = np.cumsum(hit & ~ign).astype(np.float64)
+                    fp = np.cumsum(~hit & ~ign).astype(np.float64)
+                    recall[t, k, a, m], precision[t, :, k, a, m], scores[t, :, k, a, m] = sample_pr_curve(
+                        tp, fp, score[sel], n_valid[k, a], rec)
+    return precision, recall, scores

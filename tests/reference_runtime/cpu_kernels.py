@@ -399,103 +399,28 @@ def mask_pair_intersections(det_words, det_word_off, gt_words, gt_word_off, det_
     return torch.from_numpy(out)
 
 
-_MAP_AREAS = [(0.0, 1e10), (0.0, 32.0 ** 2), (32.0 ** 2, 96.0 ** 2), (96.0 ** 2, 1e10)]
-
-
 def coco_map_match(det_box, det_score, det_label, det_counts, gt_box, gt_label, gt_crowd, gt_area, gt_counts, classes,
                    iou_thresholds, max_det_last, micro=False, masks=None, gt_area_exact=False):
-    """Stand-in for `mb200_coco_map_match(_ex)`: COCOeval.evaluateImg per (image, class, area range) with the oracle's matching
-    loop (oracle/coco_map.py::match_detections), written out as the kernel's per-detection records: class index, rank inside
-    the (image, class), 64-bit match / ignore words (bit = area * T + threshold); `npig` [K, 4]."""
-    import numpy as np
+    """Stand-in for `mb200_coco_map_match(_ex)`: the records of oracle/coco_map.py::match_records as tensors."""
+    from oracle.coco_map import match_records
 
-    from oracle.coco_map import bb_iou, match_detections
-
-    thr = np.asarray(iou_thresholds, np.float64)
-    T = len(thr)
-    cls = classes.numpy()
-    K = 1 if micro else len(cls)
-    n_det = int(sum(det_counts))
-    cat = np.zeros(n_det, np.int32)
-    rank = np.zeros(n_det, np.int32)
-    match = np.zeros(n_det, np.uint64)
-    ignore = np.zeros(n_det, np.uint64)
-    npig = np.zeros((K, 4), np.int32)
-    dbox, gbox = det_box.numpy().astype(np.float32).reshape(-1, 4), gt_box.numpy().astype(np.float32).reshape(-1, 4)
-    dscore, dlab, glab = det_score.numpy().astype(np.float32), det_label.numpy(), gt_label.numpy()
-    gcrowd = gt_crowd.numpy().astype(bool)
-    given = gt_area.numpy().astype(np.float64)
-    garea = given if gt_area_exact else np.where(given > 0, given, gbox[:, 2].astype(np.float64) * gbox[:, 3].astype(np.float64))
-    if masks is not None:
-        inter, pair_off = masks["pair_inter"].numpy(), masks["pair_off"].tolist()
-        d_marea, g_marea = masks["det_area"].numpy(), masks["gt_area"].numpy()
-    d0 = g0 = 0
-    for img, (nd, ng) in enumerate(zip(det_counts, gt_counts)):
-        dcat = np.zeros(nd, np.int64) if micro else np.searchsorted(cls, dlab[d0:d0 + nd])
-        gcat = np.zeros(ng, np.int64) if micro else np.searchsorted(cls, glab[g0:g0 + ng])
-        cat[d0:d0 + nd] = dcat
-        for c in np.unique(np.concatenate([dcat, gcat])):
-            di, gi = np.flatnonzero(dcat == c), np.flatnonzero(gcat == c)
-            order = di[np.argsort(-dscore[d0 + di], kind="mergesort")]
-            rank[d0 + order] = np.arange(len(order))
-            top = order[:max_det_last]
-            for a, (lo, hi) in enumerate(_MAP_AREAS):
-                g_ig = gcrowd[g0 + gi] | (garea[g0 + gi] < lo) | (garea[g0 + gi] > hi)
-                npig[c, a] += int((~g_ig).sum())
-                g_order = gi[np.argsort(g_ig, kind="mergesort")]
-                g_ig_sorted = np.sort(g_ig, kind="mergesort")
-                crowd_sorted = gcrowd[g0 + g_order]
-                if masks is not None:
-                    table = inter[pair_off[img]: pair_off[img] + nd * ng].reshape(nd, ng)[np.ix_(top, g_order)]
-                    da, ga = d_marea[d0 + top][:, None], g_marea[g0 + g_order][None, :]
-                    with np.errstate(divide="ignore", invalid="ignore"):
-                        ious = np.where(table > 0, table / np.where(crowd_sorted[None, :], da, da + ga - table), 0.0)
-                    d_area = d_marea[d0 + top]
-                else:
-                    ious = bb_iou(dbox[d0 + top], gbox[g0 + g_order], crowd_sorted) if len(top) and len(g_order) else np.zeros((len(top), len(g_order)))
-                    d_area = dbox[d0 + top, 2].astype(np.float64) * dbox[d0 + top, 3].astype(np.float64)
-                dtm, dt_ig = match_detections(ious, crowd_sorted, g_ig_sorted, thr)
-                outside = (d_area < lo) | (d_area > hi)
-                dt_ig = dt_ig | ((dtm == 0) & outside[None, :])
-                for t in range(T):
-                    bit = np.uint64(1) << np.uint64(a * T + t)
-                    match[d0 + top[dtm[t] > 0]] |= bit
-                    ignore[d0 + top[dt_ig[t]]] |= bit
-        d0, g0 = d0 + nd, g0 + ng
-    as_i64 = lambda x: torch.from_numpy(x.view(np.int64).copy())  # noqa: E731
+    m = {k: v.numpy() for k, v in masks.items()} if masks is not None else {}
+    cat, rank, match, ignore, npig = match_records(
+        det_box.numpy(), det_score.numpy(), det_label.numpy(), det_counts, gt_box.numpy(), gt_label.numpy(), gt_crowd.numpy(),
+        gt_area.numpy(), gt_counts, classes.numpy(), iou_thresholds, max_det_last, micro=micro, pair_inter=m.get("pair_inter"),
+        pair_off=m.get("pair_off"), det_mask_area=m.get("det_area"), gt_mask_area=m.get("gt_area"), gt_area_exact=gt_area_exact)
+    as_i64 = lambda x: torch.from_numpy(x.view("int64").copy())  # noqa: E731
     return (torch.from_numpy(cat), torch.from_numpy(rank), as_i64(match), as_i64(ignore)), torch.from_numpy(npig), torch.zeros(1, dtype=torch.int32)
 
 
 def coco_map_accumulate(det_cat, det_score, det_rank, det_match, det_ignore, npig, num_classes, class_lo, class_hi, n_iou_thr,
                         rec_thresholds, max_dets):
-    """Stand-in for `mb200_coco_map_accumulate`: COCOeval.accumulate from the per-detection records for classes [lo, hi)
-    (ties in score keep the given order), sampling with the oracle's `sample_pr_curve`."""
-    import numpy as np
+    """Stand-in for `mb200_coco_map_accumulate`: oracle/coco_map.py::accumulate_records on the records."""
+    from oracle.coco_map import accumulate_records
 
-    from oracle.coco_map import sample_pr_curve
-
-    T, R, K, M = int(n_iou_thr), len(rec_thresholds), int(num_classes), len(max_dets)
-    rec = np.asarray(rec_thresholds, np.float64)
-    precision, recall, scores = -np.ones((T, R, K, 4, M)), -np.ones((T, K, 4, M)), -np.ones((T, R, K, 4, M))
-    cat, rank = det_cat.numpy(), det_rank.numpy()
-    score = det_score.numpy().astype(np.float32).astype(np.float64)
-    match, ignore = det_match.numpy().view(np.uint64), det_ignore.numpy().view(np.uint64)
-    n_valid = npig.numpy()
-    for k in range(int(class_lo), int(class_hi)):
-        for a in range(4):
-            if n_valid[k, a] == 0:
-                continue
-            for m, max_det in enumerate(max_dets):
-                sel = np.flatnonzero((cat == k) & (rank < max_det))
-                sel = sel[np.argsort(-score[sel], kind="mergesort")]
-                for t in range(T):
-                    bit = np.uint64(1) << np.uint64(a * T + t)
-                    hit, ign = (match[sel] & bit) != 0, (ignore[sel] & bit) != 0
-                    tp = np.cumsum(hit & ~ign).astype(np.float64)
-                    fp = np.cumsum(~hit & ~ign).astype(np.float64)
-                    recall[t, k, a, m], precision[t, :, k, a, m], scores[t, :, k, a, m] = sample_pr_curve(tp, fp, score[sel],
-                                                                                                           n_valid[k, a], rec)
-    return torch.from_numpy(precision), torch.from_numpy(recall), torch.from_numpy(scores), torch.zeros(1, dtype=torch.int32)
+    out = accumulate_records(det_cat.numpy(), det_score.numpy(), det_rank.numpy(), det_match.numpy(), det_ignore.numpy(),
+                             npig.numpy(), num_classes, class_lo, class_hi, n_iou_thr, rec_thresholds, max_dets)
+    return tuple(torch.from_numpy(x) for x in out) + (torch.zeros(1, dtype=torch.int32),)
 
 
 def kl_divergence_rows(p: Tensor, q: Tensor, log_prob: bool) -> Tensor:

@@ -88,3 +88,23 @@ def test_crowd_union_is_the_detection_area():
                "iscrowd": torch.tensor([1, 0])}]
     got = _pairwise_ious(max_det=100, **_state(preds, target))
     assert got[(0, 1)].tolist() == [[pytest.approx(2 / 4), pytest.approx(2 / 12)]]
+
+
+@pytest.mark.parametrize("device", ["cpu", pytest.param("cuda:0", marks=pytest.mark.gpu)])
+def test_detection_order_nan_signed_zero_inf(device):
+    """Rows follow COCOeval's `argsort(-score, kind="mergesort")`: NaN last in input order, -0.0 and +0.0 tied in input
+    order, +-inf at the ends; the max_det cut keeps the first rows of that order."""
+    nan, inf = float("nan"), float("inf")
+    scores = [0.3, nan, 0.9, 0.9, -0.0, 0.0, -inf, inf, -0.0, nan, 0.0]
+    n = len(scores)
+    det_box = torch.tensor([[float(i), 0.0, 10.0, 10.0] for i in range(n)])
+    gt_box = torch.tensor([[0.0, 0.0, 10.0, 10.0], [3.0, 0.0, 10.0, 10.0]])
+    dev = torch.device(device)
+    for max_det in (100, 7, 2):
+        got = _pairwise_ious(det_box.to(dev), torch.tensor(scores).to(dev), torch.zeros(n, dtype=torch.int64, device=dev), [n],
+                             gt_box.to(dev), torch.zeros(2, dtype=torch.int64, device=dev), torch.zeros(2, dtype=torch.uint8, device=dev),
+                             [2], [0], False, max_det)
+        want = compute_ious([det_box.numpy()], [np.array(scores, np.float32)], [np.zeros(n, np.int64)], [gt_box.numpy()],
+                            [np.zeros(2, np.int64)], [np.zeros(2, np.int64)], [0], max_det)
+        got = {k: (v.cpu() if isinstance(v, torch.Tensor) else v) for k, v in got.items()}
+        assert _same(got, want) == 1

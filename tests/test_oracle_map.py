@@ -78,3 +78,97 @@ def test_segm_docstring_known_answer():
                 mar_100=0.2, mar_large=-1.0, mar_medium=-1.0, mar_small=0.2)
     for k, v in want.items():
         assert abs(float(r[k]) - v) < 1e-6, k
+
+
+# ---- the record-level restatement (match_records / accumulate_records) against COCOeval restated per image -------------
+def _legacy_flat_case(name):
+    from oracle.coco_map import box_convert_to_xywh
+    from tests.coco_map_cases import make_case
+
+    preds, target = synth_detection(**LEGACY_MAP_CASES[name])
+    kw = det_to_numpy(preds, target)
+    images = []
+    for i in range(len(kw["det_labels"])):
+        db, gb = box_convert_to_xywh(kw["det_boxes"][i], "xyxy"), box_convert_to_xywh(kw["gt_boxes"][i], "xyxy")
+        det = [tuple(b) + (s, lab) for b, s, lab in zip(db.tolist(), kw["det_scores"][i].tolist(), kw["det_labels"][i].tolist())]
+        gt = [tuple(b) + (lab, 0, 0.0) for b, lab in zip(gb.tolist(), kw["gt_labels"][i].tolist())]
+        images.append(dict(det=det, gt=gt))
+    return make_case(images)
+
+
+def _hand_built(name):
+    from tests.coco_map_cases import HAND_BUILT
+
+    return HAND_BUILT[name]()
+
+
+def _records_equal_coco_evaluate(case):
+    from oracle.coco_map import accumulate_records
+    from tests.coco_map_cases import coco_eval, oracle_records
+
+    cat, rank, match, ignore, npig = oracle_records(case)
+    got = accumulate_records(cat, case["det_score"], rank, match, ignore, npig, npig.shape[0], 0, npig.shape[0],
+                             len(case["iou_thr"]), case["rec_thr"], case["max_dets"])
+    want = coco_eval(case)
+    for name, g in zip(("precision", "recall", "scores"), got):
+        np.testing.assert_array_equal(g, want[name], err_msg=name)
+
+
+@pytest.mark.parametrize("name", list(LEGACY_MAP_CASES))
+def test_records_equal_coco_evaluate_legacy(name):
+    _records_equal_coco_evaluate(_legacy_flat_case(name))
+
+
+@pytest.mark.parametrize("name", ["iou_at_threshold", "equal_iou_ties", "crowd_reuse", "area_bounds", "degenerate_boxes",
+                                  "label_values", "label_values_micro", "tied_scores", "signed_zero_inf_scores", "mask_edges",
+                                  "mask_edges_micro"])
+def test_records_equal_coco_evaluate_hand_built(name):
+    _records_equal_coco_evaluate(_hand_built(name))
+
+
+def test_records_equal_coco_evaluate_nan_scores():
+    _records_equal_coco_evaluate(_hand_built("nan_scores"))
+
+
+def _order_key_rank(score, cat):
+    """csrc/cocomap.cu's per-image rank restated: coco_det_order_key (NaN -> all ones, else the inverted order key with
+    -0 -> +0), rank = number of same-class detections with a smaller key, or an equal key and a smaller index."""
+    bits = np.asarray(score, np.float32).view(np.uint32).astype(np.uint64)
+    bits = np.where(bits == 0x80000000, 0, bits)
+    key = np.where(bits & 0x80000000, ~bits & 0xFFFFFFFF, bits | 0x80000000)  # f32_order_key
+    key = np.where(np.isnan(score), 0xFFFFFFFF, ~key & 0xFFFFFFFF)
+    idx = np.arange(len(key))
+    before = (cat[None, :] == cat[:, None]) & ((key[None, :] < key[:, None]) | ((key[None, :] == key[:, None]) & (idx[None, :] < idx[:, None])))
+    return before.sum(1)
+
+
+@pytest.mark.parametrize("scores", [
+    [0.3, float("nan"), 0.9, 0.9],
+    [float("nan"), float("-inf"), float("nan"), 0.1, float("inf"), -0.0, 0.0, float("nan"), -1e-45, 1e-45],
+    [-0.0, 0.0, -0.0, 0.0, float("inf"), float("-inf")],
+])
+def test_nan_signed_zero_inf_follow_mergesort_order(scores):
+    """The kernel's order key ranks detections exactly as COCOeval's `argsort(-score, kind="mergesort")`: NaN last in input
+    order, +-0 tied, -inf just before NaN; match_records writes those ranks."""
+    from oracle.coco_map import match_records
+
+    s = np.array(scores, np.float32)
+    want = np.empty(len(s), np.int64)
+    want[np.argsort(-s, kind="mergesort")] = np.arange(len(s))
+    np.testing.assert_array_equal(_order_key_rank(s, np.zeros(len(s), np.int64)), want)
+    n = len(s)
+    box = np.tile(np.array([[0, 0, 10, 10]], np.float32), (n, 1))
+    _, rank, _, _, _ = match_records(box, s, np.zeros(n, np.int64), [n], box[:1], np.zeros(1, np.int64), np.zeros(1, np.uint8),
+                                     np.zeros(1), [1], np.array([0]), [0.5], 100)
+    np.testing.assert_array_equal(rank, want)
+
+
+def test_bb_iou_vectorised_equals_scalar_loop():
+    from oracle.coco_map import bb_iou, bb_iou_scalar
+
+    rng = np.random.default_rng(0)
+    d = np.concatenate([rng.integers(-5, 40, (60, 4)).astype(np.float32), (rng.random((60, 4)) * 50 - 5).astype(np.float32)])
+    g = np.concatenate([rng.integers(-5, 40, (30, 4)).astype(np.float32), (rng.random((30, 4)) * 50 - 5).astype(np.float32)])
+    crowd = rng.random(60) < 0.3
+    got, want = bb_iou(d, g, crowd), bb_iou_scalar(d, g, crowd)
+    assert got.tobytes() == want.tobytes()
