@@ -15,32 +15,12 @@
 
 namespace mb200 {
 
-extern void count_launch();
-
-template <typename T>
-__device__ __forceinline__ float score_to_float(T x);
-template <>
-__device__ __forceinline__ float score_to_float<float>(float x) { return x; }
-template <>
-__device__ __forceinline__ float score_to_float<__half>(__half x) { return __half2float(x); }
-template <>
-__device__ __forceinline__ float score_to_float<__nv_bfloat16>(__nv_bfloat16 x) { return __bfloat162float(x); }
-template <>
-__device__ __forceinline__ float score_to_float<double>(double x) { return (float)x; }
-
-template <typename T>
-__device__ __forceinline__ float round_to(float x) { return x; }
-template <>
-__device__ __forceinline__ float round_to<__half>(float x) { return __half2float(__float2half_rn(x)); }
-template <>
-__device__ __forceinline__ float round_to<__nv_bfloat16>(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
-
 template <typename T>
 __device__ __forceinline__ bool out_of_unit_range(T x) {
     if constexpr (sizeof(T) == 8) {
         return (x < 0.0) | (x > 1.0);
     } else {
-        const float v = score_to_float<T>(x);
+        const float v = to_f32(x);
         return (v < 0.f) | (v > 1.f);
     }
 }
@@ -88,7 +68,7 @@ struct BinArgs {
 template <typename T>
 __device__ __forceinline__ long long pred_label(const BinArgs& a, long long i, bool logits) {
     const T* __restrict__ p = reinterpret_cast<const T*>(a.preds);
-    float v = score_to_float<T>(p[i]);
+    float v = to_f32(p[i]);
     if (logits) v = round_to<T>(1.0f / (1.0f + expf(-v)));  // ATen's sigmoid: fp32 math, result stored in T
     return v > a.threshold ? 1 : 0;
 }
@@ -200,7 +180,7 @@ __device__ __forceinline__ int pred_from_value(const BinArgs& a, T x, bool logit
         if (logits) v = 1.0 / (1.0 + exp(-v));
         return v > a.threshold_d ? 1 : 0;
     } else {
-        float v = score_to_float<T>(x);
+        float v = to_f32(x);
         if (logits) v = round_to<T>(1.0f / (1.0f + expf(-v)));
         return v > a.threshold ? 1 : 0;
     }
@@ -285,7 +265,7 @@ __global__ void __launch_bounds__(256) bin_count_flat_both_kernel(BinArgs a, Bot
     bool bad_target = false, outside = false;
     const bool bracket = b.x_lo == b.x_lo;  // NaN bracket: no shortcut for this threshold
     auto count = [&](T x, long long t) {
-        const float v = score_to_float<T>(x);
+        const float v = to_f32(x);
         outside |= (v < 0.f) | (v > 1.f);  // the vote runs over EVERY score, ignored targets included, like the reference's
                                            // `torch.all((preds >= 0) * (preds <= 1))` (stat_scores.py:118-121)
         if (a.has_ignore && t == a.ignore_index) return;

@@ -10,38 +10,6 @@
 
 namespace mb200 {
 
-extern void count_launch();
-
-template <typename T>
-__device__ __forceinline__ float binned_to_float(T x);
-template <>
-__device__ __forceinline__ float binned_to_float<float>(float x) { return x; }
-template <>
-__device__ __forceinline__ float binned_to_float<__half>(__half x) { return __half2float(x); }
-template <>
-__device__ __forceinline__ float binned_to_float<__nv_bfloat16>(__nv_bfloat16 x) { return __bfloat162float(x); }
-template <>
-__device__ __forceinline__ float binned_to_float<double>(double x) { return (float)x; }
-template <typename T>
-struct CmpType { using type = float; };
-template <>
-struct CmpType<double> { using type = double; };  // fp64 scores are compared in fp64
-template <typename T>
-__device__ __forceinline__ typename CmpType<T>::type binned_load(const T* p, long long i) { return binned_to_float<T>(p[i]); }
-template <>
-__device__ __forceinline__ double binned_load<double>(const double* p, long long i) { return p[i]; }
-
-// Threshold i of a list of any float or integer dtype, exactly (integers up to 2^53).
-__device__ __forceinline__ double binned_threshold(const void* thr, int thr_dtype, long long i) {
-    switch (thr_dtype) {
-        case MB200_F32: return reinterpret_cast<const float*>(thr)[i];
-        case MB200_F16: return __half2float(reinterpret_cast<const __half*>(thr)[i]);
-        case MB200_BF16: return __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(thr)[i]);
-        case MB200_F64: return reinterpret_cast<const double*>(thr)[i];
-        default: return (double)load_label(thr, thr_dtype, i);
-    }
-}
-
 // The comparand c of threshold t for `score >= t` evaluated in dtype cmp_dtype (DESIGN §2 K4): for every score p of the
 // kernel's score type, `p >= c` in Cmp holds exactly when the reference's comparison does.
 //  * f16 / bf16: ATen casts t to the score dtype (through float, as c10::Half / c10::BFloat16 do) and compares;
@@ -51,13 +19,13 @@ __device__ __forceinline__ double binned_threshold(const void* thr, int thr_dtyp
 // Every case is a monotone function of t, so an ascending list stays ascending.
 template <typename Cmp>
 __device__ __forceinline__ Cmp binned_comparand(const void* thr, int thr_dtype, int cmp_dtype, long long i) {
-    const double t = binned_threshold(thr, thr_dtype, i);
+    const double t = load_f64(thr, thr_dtype, i);
     if constexpr (std::is_same<Cmp, double>::value) {
         return t;
     } else {
         switch (cmp_dtype) {
-            case MB200_F16: return __half2float(__float2half_rn((float)t));
-            case MB200_BF16: return __bfloat162float(__float2bfloat16_rn((float)t));
+            case MB200_F16: return round_to<__half>((float)t);
+            case MB200_BF16: return round_to<__nv_bfloat16>((float)t);
             case MB200_F64: return __double2float_ru(t);
             default: return (float)t;
         }
@@ -83,7 +51,7 @@ __global__ void __launch_bounds__(256) binned_bucket_kernel(const T* __restrict_
     extern __shared__ __align__(8) unsigned sh_cnt[];
     const int stride = nthr + 1;
     const int ncnt = C * 2 * stride;
-    typedef typename CmpType<T>::type Cmp;
+    typedef compute_t<T> Cmp;
     Cmp* sh_stage = reinterpret_cast<Cmp*>(sh_cnt + (use_smem ? ncnt : 0));
     if (thr_in_smem)
         for (int i = threadIdx.x; i < nthr; i += blockDim.x) sh_stage[i] = binned_comparand<Cmp>(thr, thr_dtype, cmp_dtype, i);
@@ -149,7 +117,7 @@ __global__ void __launch_bounds__(256) binned_bucket_kernel(const T* __restrict_
                 cc[u] = (int)(e - srow * C);
             }
             tt[u] = load_label(target, tdtype, flat ? e : srow);
-            pp[u] = binned_load<T>(preds, e);
+            pp[u] = widen(preds[e]);
         }
 #pragma unroll
         for (int u = 0; u < kUnroll; ++u) commit(cc[u], tt[u], pp[u]);
@@ -161,7 +129,7 @@ __global__ void __launch_bounds__(256) binned_bucket_kernel(const T* __restrict_
             srow = small ? (long long)((unsigned)i / (unsigned)C) : i / C;
             c = (int)(i - srow * C);
         }
-        commit(c, load_label(target, tdtype, flat ? i : srow), binned_load<T>(preds, i));
+        commit(c, load_label(target, tdtype, flat ? i : srow), widen(preds[i]));
     }
     if (use_smem) {
         __syncthreads();
@@ -418,7 +386,7 @@ static int binned_update_impl(int multilabel, const void* preds, int preds_dtype
     }
     with_float_type(preds_dtype, [&](auto t) {
         using T = typename decltype(t)::type;
-        using Cmp = typename CmpType<T>::type;
+        using Cmp = compute_t<T>;
         // comparands in shared memory when they fit beside the counters under the 48 KB that needs no opt-in: always for
         // float comparands (40 KB + 2048 * 4 B), not for 2048 double ones next to more than 32 KB of counters
         const size_t thr_bytes = (size_t)num_thresholds * sizeof(Cmp);

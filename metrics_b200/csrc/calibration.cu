@@ -23,34 +23,7 @@
 
 namespace mb200 {
 
-extern void count_launch();
-
 namespace {
-
-// ---- element access: f32 / f16 / bf16 compute in float (exact widening), f64 in double ---------------------------------
-template <typename T>
-struct Cal {
-    using A = float;
-};
-template <>
-struct Cal<double> {
-    using A = double;
-};
-__device__ __forceinline__ float widen(float x) { return x; }
-__device__ __forceinline__ float widen(__half x) { return __half2float(x); }
-__device__ __forceinline__ float widen(__nv_bfloat16 x) { return __bfloat162float(x); }
-__device__ __forceinline__ double widen(double x) { return x; }
-// round an A to T and widen it back: the value a tensor of dtype T would hold
-template <typename T>
-__device__ __forceinline__ typename Cal<T>::A round_to(typename Cal<T>::A x);
-template <>
-__device__ __forceinline__ float round_to<float>(float x) { return x; }
-template <>
-__device__ __forceinline__ float round_to<__half>(float x) { return __half2float(__float2half_rn(x)); }
-template <>
-__device__ __forceinline__ float round_to<__nv_bfloat16>(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
-template <>
-__device__ __forceinline__ double round_to<double>(double x) { return x; }
 
 __device__ __forceinline__ float exp_a(float x) { return expf(x); }
 __device__ __forceinline__ double exp_a(double x) { return exp(x); }
@@ -138,8 +111,7 @@ __global__ void __launch_bounds__(256, kIter >= 32 ? 2 : 3) top_label_spec_kerne
                 pending[r] = 1;
             }
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(kFull, m, o));
+        m = warp_max(m);
         float s = 0.f;
 #pragma unroll
         for (int it = 0; it < kIter; ++it) {
@@ -149,8 +121,7 @@ __global__ void __launch_bounds__(256, kIter >= 32 ? 2 : 3) top_label_spec_kerne
                 s += v[it];
             }
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(kFull, s, o);
+        s = warp_sum(s);
         // Top label of the softmax rounded to T (in case the batch holds logits).  Without a NaN in the row every e lies in
         // [0, 1] and s in [1, C <= 1024], so the largest probability round(1 / s) and half of it are normal numbers of T: a
         // quotient of e < 0.5 rounds to at most half the maximum and cannot win, and the division is skipped for it (the
@@ -201,7 +172,7 @@ template <typename T>
 __global__ void __launch_bounds__(256) top_label_vote_kernel(const T* __restrict__ x, const void* __restrict__ target, int tdtype,
                                                              int n, int C, int has_ignore, long long ignore_index,
                                                              unsigned* __restrict__ vote, unsigned* __restrict__ err) {
-    using A = typename Cal<T>::A;
+    using A = compute_t<T>;
     const int lane = threadIdx.x & 31;
     const int wpb = blockDim.x >> 5;
     bool voted = false;
@@ -228,7 +199,7 @@ __global__ void __launch_bounds__(256) top_label_rows_kernel(const T* __restrict
                                                              int n, int C, int has_ignore, long long ignore_index,
                                                              const unsigned* __restrict__ vote, float* __restrict__ conf,
                                                              float* __restrict__ acc) {
-    using A = typename Cal<T>::A;
+    using A = compute_t<T>;
     const bool apply = (*vote) != 0u;
     const int lane = threadIdx.x & 31;
     const int wpb = blockDim.x >> 5;
@@ -252,12 +223,10 @@ __global__ void __launch_bounds__(256) top_label_rows_kernel(const T* __restrict
         } else {
             A m = -INFINITY;
             for (int c = lane; c < C; c += 32) m = max_a(m, widen(row[c]));
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) m = max_a(m, __shfl_xor_sync(kFull, m, o));
+            m = warp_max(m);
             A s = 0;
             for (int c = lane; c < C; c += 32) s += exp_a(widen(row[c]) - m);
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(kFull, s, o);
+            s = warp_sum(s);
             for (int c = lane; c < C; c += 32) {
                 const A q = round_to<T>(exp_a(widen(row[c]) - m) / s);
                 if (beats(q, c, bv, bi)) {
@@ -298,23 +267,13 @@ int bin_warps(int slots) {
     return 1;
 }
 
-__device__ __forceinline__ double load_value(const void* p, int dtype, long long i) {
-    switch (dtype) {
-        case MB200_F32: return reinterpret_cast<const float*>(p)[i];
-        case MB200_F16: return __half2float(reinterpret_cast<const __half*>(p)[i]);
-        case MB200_BF16: return __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p)[i]);
-        case MB200_F64: return reinterpret_cast<const double*>(p)[i];
-        default: return (double)load_label(p, dtype, i);
-    }
-}
-
 // Block b bins rows [b * chunk, min(n, (b + 1) * chunk)); warp w of W takes 32 rows at a time, W * 32 apart.  Partials of
 // block b go to part[(b * 3 + k) * slots + s]: k = 0 count (int64 bits), 1 confidence sum, 2 accuracy sum.
 template <typename T>
 __global__ void __launch_bounds__(256) bin_partials_kernel(const T* __restrict__ conf, const void* __restrict__ accp, int acc_dtype,
                                                            long long n, long long chunk, const T* __restrict__ bounds,
                                                            int slots, double* __restrict__ part) {
-    using A = typename Cal<T>::A;
+    using A = compute_t<T>;
     extern __shared__ __align__(16) unsigned char smem[];
     const int W = blockDim.x >> 5;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -352,7 +311,7 @@ __global__ void __launch_bounds__(256) bin_partials_kernel(const T* __restrict__
             }
             bin = lo - 1;  // -1 only for a negative confidence, which normalised scores never are: not counted
             cd = (double)xv;
-            ad = (double)round_to<T>((A)load_value(accp, acc_dtype, i));
+            ad = (double)round_to<T>((A)load_f64(accp, acc_dtype, i));
         }
         const unsigned peers = __match_any_sync(kFull, bin);
         stage[lane] = cd;
@@ -470,7 +429,7 @@ int launch_top_label(const void* preds, const void* target, int tdtype, int n, i
 template <typename T>
 int launch_bin_sums(const void* confidences, const void* accuracies, int acc_dtype, int64_t n, const void* boundaries, int slots,
                     int64_t* count, double* sum_conf, double* sum_acc, double* part, cudaStream_t st) {
-    using A = typename Cal<T>::A;
+    using A = compute_t<T>;
     const int W = bin_warps<A>(slots);
     const size_t smem = bin_smem_bytes<A>(W, slots);
     MB200_REQUIRE(smem <= (size_t)kBinSmemCap, "n_bins = %d needs %zu bytes of shared memory per warp", slots - 1, smem);

@@ -23,8 +23,6 @@
 
 namespace mb200 {
 
-extern void count_launch();
-
 constexpr int kMapAreas = 4;
 constexpr int kMapMaxThr = 16;  // T <= 16 so that area*T + thr fits a 64-bit word
 constexpr int kGtmWords = 4;    // "matched" bit mask kept in registers: <= 256 ground truths of one class in one image;

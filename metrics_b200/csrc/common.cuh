@@ -11,6 +11,7 @@
 
 #include <type_traits>
 #include <unordered_map>
+#include <utility>
 
 #include "../../include/metrics_b200.h"
 
@@ -23,6 +24,7 @@ constexpr unsigned kFull = 0xffffffffu;
 void set_error(const char* fmt, ...);
 int check_cuda(cudaError_t e, const char* what);
 int sm_count();  // cached multiprocessor count of the current device
+void count_launch();  // adds one to mb200_launch_count(): called once per kernel launch
 
 #define MB200_CUDA_OK(expr)                                      \
     do {                                                         \
@@ -147,6 +149,78 @@ __device__ __forceinline__ unsigned long long f64_order_key(double v) {
     if ((b & 0x7fffffffffffffffull) > 0x7ff0000000000000ull) return ~0ull;
     if (b == 0x8000000000000000ull) b = 0ull;
     return (b & 0x8000000000000000ull) ? ~b : (b | 0x8000000000000000ull);
+}
+
+// ---- score types ----------------------------------------------------------------------------------------------------
+// What a kernel does with one value of a score type T (float, __half, __nv_bfloat16, double) once with_float_type has
+// picked T.  half and bfloat16 widen exactly to float and compute in float; double computes in double.  Keys and score
+// comparisons see every type as float32 (to_f32), as ATen compares half and bfloat16; float64 is rounded to float there.
+__device__ __forceinline__ float widen(float v) { return v; }
+__device__ __forceinline__ float widen(__half v) { return __half2float(v); }
+__device__ __forceinline__ float widen(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ double widen(double v) { return v; }
+template <typename T>
+using compute_t = decltype(widen(std::declval<T>()));
+
+template <typename T>
+__device__ __forceinline__ float to_f32(T v) { return (float)widen(v); }
+
+// a computed value stored in T, rounded to nearest
+template <typename T>
+__device__ __forceinline__ T narrow(compute_t<T> x) {
+    if constexpr (std::is_same_v<T, __half>) return __float2half_rn(x);
+    else if constexpr (std::is_same_v<T, __nv_bfloat16>) return __float2bfloat16_rn(x);
+    else return x;
+}
+// the value a tensor of dtype T would hold
+template <typename T>
+__device__ __forceinline__ compute_t<T> round_to(compute_t<T> x) { return widen(narrow<T>(x)); }
+
+// element i of a tensor of any float or integer tag, exactly (integers up to 2^53)
+__device__ __forceinline__ double load_f64(const void* p, int dtype, long long i) {
+    switch (dtype) {
+        case MB200_F32: return reinterpret_cast<const float*>(p)[i];
+        case MB200_F16: return widen(reinterpret_cast<const __half*>(p)[i]);
+        case MB200_BF16: return widen(reinterpret_cast<const __nv_bfloat16*>(p)[i]);
+        case MB200_F64: return reinterpret_cast<const double*>(p)[i];
+        default: return (double)load_label(p, dtype, i);
+    }
+}
+
+// ascending sort of this key == descending sort of the score; NaN first (torch.argsort(descending=True) puts NaN first)
+__device__ __forceinline__ unsigned f32_desc_key(float v) { return ~f32_order_key(v); }
+
+// butterfly over the 32 lanes (offsets 16, 8, 4, 2, 1): every lane ends with the same sum / maximum
+template <typename V>
+__device__ __forceinline__ V warp_sum(V v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
+    return v;
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(kFull, v, o));
+    return v;
+}
+__device__ __forceinline__ double warp_max(double v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(kFull, v, o));
+    return v;
+}
+
+// ---- key tiles ------------------------------------------------------------------------------------------------------
+// This CTA's 32 x 32 tile of [n, C] row-major scores (samples from blockIdx.x * 32, classes from blockIdx.y * 32) as
+// tile[sample][class] = f32_desc_key(to_f32(score)), read along the class dimension by 256 threads.  Both key-packing
+// transposes, the exact curves' (curve.cu) and the class-sharded peer exchange's (peer.cu), load through it: the sharded
+// curves rely on the two producing the same keys.  Entries outside [n, C] are not written.
+template <typename T>
+__device__ __forceinline__ void load_desc_key_tile(const T* __restrict__ preds, int n, int C, unsigned (&tile)[32][33]) {
+    const int n0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+    for (int j = ty; j < 32; j += 8) {
+        const int nn = n0 + j, cc = c0 + tx;
+        if (nn < n && cc < C) tile[j][tx] = f32_desc_key(to_f32(preds[(size_t)nn * C + cc]));
+    }
 }
 
 // Opt a kernel into more than 48 KB of dynamic shared memory.  The attribute is per (function, device): remember which

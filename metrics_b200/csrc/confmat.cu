@@ -190,8 +190,6 @@ __global__ void __launch_bounds__(kRowThreads) labels_kernel(RowArgs a, int pred
 // =====================================================================================================
 // Host dispatch
 // =====================================================================================================
-extern void count_launch();
-
 static inline int grid_for(long long work_items, int items_per_block, int max_blocks) {
     long long g = (work_items + items_per_block - 1) / items_per_block;
     if (g < 1) g = 1;

@@ -20,34 +20,9 @@
 
 namespace mb200 {
 
-extern void count_launch();
-
 // =====================================================================================================
 // helpers
 // =====================================================================================================
-template <typename T>
-__device__ __forceinline__ float to_float(T x);
-template <>
-__device__ __forceinline__ float to_float<float>(float x) { return x; }
-template <>
-__device__ __forceinline__ float to_float<__half>(__half x) { return __half2float(x); }
-template <>
-__device__ __forceinline__ float to_float<__nv_bfloat16>(__nv_bfloat16 x) { return __bfloat162float(x); }
-template <>
-__device__ __forceinline__ float to_float<double>(double x) { return (float)x; }
-
-template <typename T>
-__device__ __forceinline__ T from_float(float x);
-template <>
-__device__ __forceinline__ float from_float<float>(float x) { return x; }
-template <>
-__device__ __forceinline__ __half from_float<__half>(float x) { return __float2half_rn(x); }
-template <>
-__device__ __forceinline__ __nv_bfloat16 from_float<__nv_bfloat16>(float x) { return __float2bfloat16_rn(x); }
-
-// ascending sort of this key == descending sort of the score; NaN first (torch.argsort(descending=True) puts NaN first)
-__device__ __forceinline__ unsigned desc_key(float v) { return ~f32_order_key(v); }
-
 // Runs the reference splits.  It finds thresholds with where(preds[1:] - preds[:-1]): NaN - NaN and inf - inf are NaN, so
 // every NaN, +inf or -inf score ends its own group.  Their desc keys sit at the two ends of the key range, next to the
 // NaN payloads no score maps to: NaN 0, +inf 0x007fffff, -inf 0xff800000 (64-bit: 0, 0x000fffffffffffff,
@@ -93,7 +68,7 @@ __device__ __forceinline__ double score_of_key(unsigned long long k) {
 template <typename T>
 struct KeyOf {
     using type = unsigned;
-    static __device__ __forceinline__ unsigned make(T v) { return desc_key(to_float<T>(v)); }
+    static __device__ __forceinline__ unsigned make(T v) { return f32_desc_key(to_f32(v)); }
 };
 template <>
 struct KeyOf<double> {
@@ -124,14 +99,14 @@ __global__ void __launch_bounds__(256) range_flag_kernel(const T* __restrict__ x
         const T* e = reinterpret_cast<const T*>(&q);
 #pragma unroll
         for (int k = 0; k < kVec; ++k) {
-            const float v = to_float<T>(e[k]);
+            const float v = to_f32(e[k]);
             bad |= (v < 0.f) | (v > 1.f);
         }
     }
     const long long tail0 = head + nvec * kVec;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < head + (n - tail0); i += (long long)gridDim.x * blockDim.x) {
         const long long j = i < head ? i : tail0 + (i - head);
-        const float v = to_float<T>(x[j]);
+        const float v = to_f32(x[j]);
         bad |= (v < 0.f) | (v > 1.f);
     }
     if (__any_sync(kFull, bad) && (threadIdx.x & 31) == 0) atomicOr(flag, 1u);
@@ -152,8 +127,8 @@ __global__ void __launch_bounds__(256) sigmoid_if_kernel(const T* __restrict__ x
     const bool apply = (*flag) != 0u;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
         if (apply) {
-            const float v = to_float<T>(x[i]);
-            out[i] = from_float<T>(sigmoid_f32(v));  // fp32 math, rounded to T like ATen's sigmoid
+            const float v = to_f32(x[i]);
+            out[i] = narrow<T>(sigmoid_f32(v));  // fp32 math, rounded to T like ATen's sigmoid
         } else {
             out[i] = x[i];
         }
@@ -198,7 +173,7 @@ __global__ void __launch_bounds__(256) sigmoid_spec_kernel(const T* __restrict__
                 const T* e = reinterpret_cast<const T*>(&q[k]);
 #pragma unroll
                 for (int j = 0; j < kVec; ++j) {
-                    const float f = to_float<T>(e[j]);
+                    const float f = to_f32(e[j]);
                     outside |= (f < 0.f) | (f > 1.f);
                 }
             }
@@ -206,7 +181,7 @@ __global__ void __launch_bounds__(256) sigmoid_spec_kernel(const T* __restrict__
         const bool last = tile == ntiles - 1;
         if (last)  // the (< one vector) scalar tail belongs to the last tile
             for (long long i = nvec * kVec + threadIdx.x; i < n; i += 256) {
-                const float f = to_float<T>(x[i]);
+                const float f = to_f32(x[i]);
                 outside |= (f < 0.f) | (f > 1.f);
             }
         const bool apply = kFix ? true : (__syncthreads_or(outside) != 0);
@@ -225,14 +200,14 @@ __global__ void __launch_bounds__(256) sigmoid_spec_kernel(const T* __restrict__
                 if (apply) {
                     T* e = reinterpret_cast<T*>(&q[k]);
 #pragma unroll
-                    for (int j = 0; j < kVec; ++j) e[j] = from_float<T>(sigmoid_f32(to_float<T>(e[j])));
+                    for (int j = 0; j < kVec; ++j) e[j] = narrow<T>(sigmoid_f32(to_f32(e[j])));
                 }
                 ov[v] = q[k];
             }
         }
         if (last)
             for (long long i = nvec * kVec + threadIdx.x; i < n; i += 256)
-                out[i] = apply ? from_float<T>(sigmoid_f32(to_float<T>(x[i]))) : x[i];
+                out[i] = apply ? narrow<T>(sigmoid_f32(to_f32(x[i]))) : x[i];
     }
 }
 
@@ -255,7 +230,7 @@ __global__ void __launch_bounds__(1024) sigmoid_if_small_kernel(const T* __restr
                 const double d = (double)v[k];
                 bad |= (d < 0.0) | (d > 1.0);
             } else {
-                const float f = to_float<T>(v[k]);
+                const float f = to_f32(v[k]);
                 bad |= (f < 0.f) | (f > 1.f);
             }
         }
@@ -270,7 +245,7 @@ __global__ void __launch_bounds__(1024) sigmoid_if_small_kernel(const T* __restr
             } else if constexpr (sizeof(T) == 8) {
                 out[i] = (T)(1.0 / (1.0 + exp(-(double)v[k])));
             } else {
-                out[i] = from_float<T>(sigmoid_f32(to_float<T>(v[k])));
+                out[i] = narrow<T>(sigmoid_f32(to_f32(v[k])));
             }
         }
     }
@@ -292,14 +267,12 @@ __global__ void __launch_bounds__(256) softmax_if_kernel(const T* __restrict__ x
             continue;
         }
         float m = -INFINITY;
-        for (int c = lane; c < C; c += 32) m = fmaxf(m, to_float<T>(row[c]));
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(kFull, m, o));
+        for (int c = lane; c < C; c += 32) m = fmaxf(m, to_f32(row[c]));
+        m = warp_max(m);
         float s = 0.f;
-        for (int c = lane; c < C; c += 32) s += expf(to_float<T>(row[c]) - m);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(kFull, s, o);
-        for (int c = lane; c < C; c += 32) orow[c] = from_float<T>(expf(to_float<T>(row[c]) - m) / s);
+        for (int c = lane; c < C; c += 32) s += expf(to_f32(row[c]) - m);
+        s = warp_sum(s);
+        for (int c = lane; c < C; c += 32) orow[c] = narrow<T>(expf(to_f32(row[c]) - m) / s);
     }
 }
 
@@ -327,7 +300,7 @@ __global__ void __launch_bounds__(256, 3) softmax_spec_kernel(const T* __restric
         for (int it = 0; it < kIter; ++it) {
             const int c = lane + 32 * it;
             if (c < C) {
-                v[it] = to_float<T>(row[c]);
+                v[it] = to_f32(row[c]);
                 outside |= (v[it] < 0.f) | (v[it] > 1.f);
                 m = fmaxf(m, v[it]);
             }
@@ -345,12 +318,11 @@ __global__ void __launch_bounds__(256, 3) softmax_spec_kernel(const T* __restric
 #pragma unroll
             for (int it = 0; it < kIter; ++it) {
                 const int c = lane + 32 * it;
-                if (c < C) orow[c] = from_float<T>(v[it]);
+                if (c < C) orow[c] = narrow<T>(v[it]);
             }
             continue;
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(kFull, m, o));
+        m = warp_max(m);
         float s = 0.f;
 #pragma unroll
         for (int it = 0; it < kIter; ++it) {
@@ -360,12 +332,11 @@ __global__ void __launch_bounds__(256, 3) softmax_spec_kernel(const T* __restric
                 s += v[it];
             }
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(kFull, s, o);
+        s = warp_sum(s);
 #pragma unroll
         for (int it = 0; it < kIter; ++it) {
             const int c = lane + 32 * it;
-            if (c < C) orow[c] = from_float<T>(v[it] / s);
+            if (c < C) orow[c] = narrow<T>(v[it] / s);
         }
     }
 }
@@ -386,12 +357,10 @@ __global__ void __launch_bounds__(256) softmax_if_kernel<double>(const double* _
         }
         double m = -INFINITY;
         for (int c = lane; c < C; c += 32) m = fmax(m, row[c]);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(kFull, m, o));
+        m = warp_max(m);
         double s = 0.0;
         for (int c = lane; c < C; c += 32) s += exp(row[c] - m);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(kFull, s, o);
+        s = warp_sum(s);
         for (int c = lane; c < C; c += 32) orow[c] = exp(row[c] - m) / s;
     }
 }
@@ -399,7 +368,7 @@ __global__ void __launch_bounds__(256) softmax_if_kernel<double>(const double* _
 // =====================================================================================================
 // key packing
 // =====================================================================================================
-// binary: keys[i] = desc_key(preds[i]), labels[i] = (target[i] == pos_label)
+// binary: keys[i] = f32_desc_key(preds[i]), labels[i] = (target[i] == pos_label)
 // kBit0 (scores promised to be non-negative or NaN — in particular everything normalize_logits_if_needed returns): their
 // 32-bit keys use 31 bits (no sign; NaN -> 0), so the label rides in bit 0 of the key and the sort moves 4-byte keys only
 // (radix_sort_passes_bit0); a negative score (other than -0) raises MB200_FLAG_PREDS_RANGE.
@@ -542,13 +511,10 @@ template <typename T>
 __global__ void __launch_bounds__(256) pack_keys_kernel(const T* __restrict__ preds, int n, int C,
                                                         unsigned* __restrict__ keys) {
     __shared__ unsigned tile[32][33];
+    load_desc_key_tile(preds, n, C, tile);
+    __syncthreads();
     const int n0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-    for (int j = ty; j < 32; j += 8) {
-        const int nn = n0 + j, cc = c0 + tx;
-        if (nn < n && cc < C) tile[j][tx] = desc_key(to_float<T>(preds[(size_t)nn * C + cc]));
-    }
-    __syncthreads();
     for (int j = ty; j < 32; j += 8) {
         const int cc = c0 + j, nn = n0 + tx;
         if (nn < n && cc < C) keys[(size_t)cc * n + nn] = tile[tx][j];

@@ -17,25 +17,6 @@
 
 namespace mb200 {
 
-extern void count_launch();
-
-template <typename T>
-__device__ __forceinline__ float fz_to_float(T x);
-template <>
-__device__ __forceinline__ float fz_to_float<float>(float x) { return x; }
-template <>
-__device__ __forceinline__ float fz_to_float<__half>(__half x) { return __half2float(x); }
-template <>
-__device__ __forceinline__ float fz_to_float<__nv_bfloat16>(__nv_bfloat16 x) { return __bfloat162float(x); }
-template <typename T>
-__device__ __forceinline__ T fz_from_float(float x);
-template <>
-__device__ __forceinline__ float fz_from_float<float>(float x) { return x; }
-template <>
-__device__ __forceinline__ __half fz_from_float<__half>(float x) { return __float2half_rn(x); }
-template <>
-__device__ __forceinline__ __nv_bfloat16 fz_from_float<__nv_bfloat16>(float x) { return __float2bfloat16_rn(x); }
-
 constexpr int kFusedThreads = 256;
 
 template <typename T, int kIter, bool kI64>
@@ -57,7 +38,7 @@ __global__ void __launch_bounds__(kFusedThreads) stats_softmax_kernel(const T* _
 #pragma unroll
         for (int it = 0; it < kIter; ++it) {
             const int c = lane + 32 * it;
-            v[it] = c < C ? fz_to_float<T>(row[c]) : -INFINITY;
+            v[it] = c < C ? to_f32(row[c]) : -INFINITY;
         }
         // ---- argmax (order keys: NaN largest, -0 == +0; first index among equals) + range vote + row maximum ----
         unsigned best_key = 0u;
@@ -75,8 +56,7 @@ __global__ void __launch_bounds__(kFusedThreads) stats_softmax_kernel(const T* _
         }
         const unsigned kmax = __reduce_max_sync(kFull, best_idx == 0x7fffffff ? 0u : best_key);
         const int p = (int)__reduce_min_sync(kFull, (best_idx != 0x7fffffff && best_key == kmax) ? (unsigned)best_idx : 0x7fffffffu);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(kFull, m, o));
+        m = warp_max(m);
         // ---- softmax, K6's order: lane-strided partial sums, butterfly ----
         float s = 0.f;
 #pragma unroll
@@ -87,13 +67,12 @@ __global__ void __launch_bounds__(kFusedThreads) stats_softmax_kernel(const T* _
                 s += v[it];
             }
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(kFull, s, o);
+        s = warp_sum(s);
         T* __restrict__ orow = probs + (size_t)r * C;
 #pragma unroll
         for (int it = 0; it < kIter; ++it) {
             const int c = lane + 32 * it;
-            if (c < C) orow[c] = fz_from_float<T>(v[it] / s);
+            if (c < C) orow[c] = narrow<T>(v[it] / s);
         }
         // ---- stat scores ----
         if ((unsigned long long)t >= (unsigned long long)C) {

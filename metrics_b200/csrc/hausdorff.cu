@@ -29,8 +29,6 @@
 
 namespace mb200 {
 
-extern void count_launch();
-
 namespace {
 
 constexpr int kThreads = 256;

@@ -10,36 +10,6 @@
 
 namespace mb200 {
 
-extern void count_launch();
-
-template <typename T>
-__device__ __forceinline__ float kl_load(const T* p, long long i);
-template <>
-__device__ __forceinline__ float kl_load<float>(const float* p, long long i) { return p[i]; }
-template <>
-__device__ __forceinline__ float kl_load<__half>(const __half* p, long long i) { return __half2float(p[i]); }
-template <>
-__device__ __forceinline__ float kl_load<__nv_bfloat16>(const __nv_bfloat16* p, long long i) { return __bfloat162float(p[i]); }
-
-template <typename T>
-__device__ __forceinline__ void kl_store(T* out, long long i, double v);
-template <>
-__device__ __forceinline__ void kl_store<float>(float* out, long long i, double v) { out[i] = (float)v; }
-template <>
-__device__ __forceinline__ void kl_store<__half>(__half* out, long long i, double v) { out[i] = __float2half_rn((float)v); }
-template <>
-__device__ __forceinline__ void kl_store<__nv_bfloat16>(__nv_bfloat16* out, long long i, double v) {
-    out[i] = __float2bfloat16_rn((float)v);
-}
-template <>
-__device__ __forceinline__ void kl_store<double>(double* out, long long i, double v) { out[i] = v; }
-
-__device__ __forceinline__ double warp_sum(double v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-    return v;
-}
-
 // f32 / f16 / bf16: elementwise in float
 template <typename T>
 __global__ void __launch_bounds__(256) kl_rows_kernel(const T* __restrict__ p, const T* __restrict__ q, long long n, int d,
@@ -85,29 +55,29 @@ __global__ void __launch_bounds__(256) kl_rows_kernel(const T* __restrict__ p, c
                     }
                 }
                 acc = warp_sum(acc);
-                if (lane == 0) kl_store<T>(out, r, acc);
+                if (lane == 0) out[r] = narrow<T>((float)acc);
                 continue;
             }
         }
         if (log_prob) {
 #pragma unroll 4
             for (int j = lane; j < d; j += 32) {
-                const float a = kl_load<T>(pr, j), b = kl_load<T>(qr, j);
+                const float a = widen(pr[j]), b = widen(qr[j]);
                 acc += (double)(expf(a) * (a - b));
             }
         } else {
             double sp = 0.0, sq = 0.0;
 #pragma unroll 8
-            for (int j = lane; j < d; j += 32) sp += (double)kl_load<T>(pr, j), sq += (double)kl_load<T>(qr, j);
+            for (int j = lane; j < d; j += 32) sp += (double)widen(pr[j]), sq += (double)widen(qr[j]);
             const float fp = (float)warp_sum(sp), fq = (float)warp_sum(sq);
 #pragma unroll 4
             for (int j = lane; j < d; j += 32) {
-                const float a = kl_load<T>(pr, j) / fp, b = kl_load<T>(qr, j) / fq;
+                const float a = widen(pr[j]) / fp, b = widen(qr[j]) / fq;
                 if (a != 0.f) acc += (double)(a * logf(a / b));  // a NaN `a` takes this branch too, like `res[x == 0] = 0`
             }
         }
         acc = warp_sum(acc);
-        if (lane == 0) kl_store<T>(out, r, acc);
+        if (lane == 0) out[r] = narrow<T>((float)acc);
     }
 }
 

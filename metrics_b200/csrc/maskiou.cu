@@ -12,8 +12,6 @@
 
 namespace mb200 {
 
-extern void count_launch();
-
 // 16 mask bytes (any non-zero value = set) -> 16 bits, pixel order
 __device__ __forceinline__ unsigned nibble_of(unsigned x) {
     unsigned t = x | (x >> 4);

@@ -36,8 +36,6 @@
 
 namespace mb200 {
 
-extern void count_launch();
-
 namespace {
 
 constexpr int kThreads = 256;

@@ -22,19 +22,6 @@
 
 namespace mb200 {
 
-extern void count_launch();
-
-__device__ __forceinline__ unsigned peer_desc_key(float v) { return ~f32_order_key(v); }
-
-template <typename T>
-__device__ __forceinline__ float peer_to_float(T x);
-template <>
-__device__ __forceinline__ float peer_to_float<float>(float x) { return x; }
-template <>
-__device__ __forceinline__ float peer_to_float<__half>(__half x) { return __half2float(x); }
-template <>
-__device__ __forceinline__ float peer_to_float<__nv_bfloat16>(__nv_bfloat16 x) { return __bfloat162float(x); }
-
 // [n, C] row-major scores -> keys of class c at peer (c / cpr): base + keys_off + ((c % cpr) * n_total + col_off + i) * 4.
 // 32 x 32 shared-memory tile transpose: coalesced 128-byte reads along the class dimension, coalesced 128-byte stores along
 // the sample dimension (one store instruction of a warp = one class row segment = one NVLink write of 128 B).
@@ -43,13 +30,10 @@ __global__ void __launch_bounds__(256) pack_keys_put_kernel(const T* __restrict_
                                                             long long n_total, long long col_off,
                                                             void* const* __restrict__ peer_bases, long long keys_off) {
     __shared__ unsigned tile[32][33];
+    load_desc_key_tile(preds, n, C, tile);
+    __syncthreads();
     const int n0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-    for (int j = ty; j < 32; j += 8) {
-        const int nn = n0 + j, cc = c0 + tx;
-        if (nn < n && cc < C) tile[j][tx] = peer_desc_key(peer_to_float<T>(preds[(size_t)nn * C + cc]));
-    }
-    __syncthreads();
     for (int j = ty; j < 32; j += 8) {
         const int cc = c0 + j, nn = n0 + tx;
         if (nn < n && cc < C) {

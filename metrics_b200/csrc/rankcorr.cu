@@ -27,8 +27,6 @@
 
 namespace mb200 {
 
-extern void count_launch();
-
 namespace {
 
 typedef unsigned long long u64;

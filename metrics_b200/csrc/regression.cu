@@ -12,19 +12,6 @@
 
 namespace mb200 {
 
-extern void count_launch();
-
-template <typename T>
-__device__ __forceinline__ double load_as_double(const T* p, long long i);
-template <>
-__device__ __forceinline__ double load_as_double<float>(const float* p, long long i) { return p[i]; }
-template <>
-__device__ __forceinline__ double load_as_double<double>(const double* p, long long i) { return p[i]; }
-template <>
-__device__ __forceinline__ double load_as_double<__half>(const __half* p, long long i) { return __half2float(p[i]); }
-template <>
-__device__ __forceinline__ double load_as_double<__nv_bfloat16>(const __nv_bfloat16* p, long long i) { return __bfloat162float(p[i]); }
-
 // grid.x CTAs of 256 threads laid out as rows x cols_per_block; grid.y tiles the columns.
 template <typename T, bool kDouble, bool kTweedie = false>
 __global__ void __launch_bounds__(256) reg_partial_kernel(const T* __restrict__ preds, const T* __restrict__ target,
@@ -42,12 +29,11 @@ __global__ void __launch_bounds__(256) reg_partial_kernel(const T* __restrict__ 
             const long long i = r * d + c;
             if (kDouble) {
                 double out[kRegMaxK];
-                reg_terms<double, kTweedie>(op, load_as_double<T>(preds, i), load_as_double<T>(target, i), param, eps, out);
+                reg_terms<double, kTweedie>(op, (double)widen(preds[i]), (double)widen(target[i]), param, eps, out);
                 for (int k = 0; k < K; ++k) acc[k] += out[k];
             } else {
                 float out[kRegMaxK];
-                reg_terms<float, kTweedie>(op, (float)load_as_double<T>(preds, i), (float)load_as_double<T>(target, i),
-                                           (float)param, (float)eps, out);
+                reg_terms<float, kTweedie>(op, to_f32(preds[i]), to_f32(target[i]), (float)param, (float)eps, out);
                 for (int k = 0; k < K; ++k) acc[k] += (double)out[k];
             }
         }
@@ -92,8 +78,7 @@ __global__ void __launch_bounds__(kRegFlatThreads) reg_flat_kernel(const T* __re
             for (int k = 0; k < K; ++k) acc[k] += out[k];
         } else {
             float out[kRegMaxK];
-            reg_terms<float, kTweedie>(op, (float)load_as_double<T>(&pv, 0), (float)load_as_double<T>(&tv, 0), (float)param,
-                                       (float)eps, out);
+            reg_terms<float, kTweedie>(op, to_f32(pv), to_f32(tv), (float)param, (float)eps, out);
             for (int k = 0; k < K; ++k) acc[k] += (double)out[k];
         }
     };

@@ -25,8 +25,6 @@
 
 namespace mb200 {
 
-extern void count_launch();
-
 namespace {
 
 constexpr int kThreads = 256;
@@ -41,8 +39,6 @@ typedef unsigned long long u64;
 __device__ __forceinline__ float load_target(const void* t, int dtype, long long i) {
     return dtype == MB200_F32 ? reinterpret_cast<const float*>(t)[i] : (float)reinterpret_cast<const long long*>(t)[i];
 }
-__device__ __forceinline__ unsigned score_key(float v) { return ~f32_order_key(v); }  // ascending sort = descending score
-
 int bytes_of(u64 v) {
     int b = 0;
     while (v) ++b, v >>= 8;
@@ -76,14 +72,14 @@ __global__ void __launch_bounds__(kThreads) range_kernel(const long long* __rest
 __global__ void pack_narrow_kernel(const long long* __restrict__ idx, const float* __restrict__ preds, const void* target,
                                    int tdtype, long long n, long long lo, u64* __restrict__ keys, unsigned* __restrict__ vals) {
     for (long long i = blockIdx.x * (long long)kThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kThreads) {
-        keys[i] = ((u64)(idx[i] - lo) << 32) | score_key(preds[i]);
+        keys[i] = ((u64)(idx[i] - lo) << 32) | f32_desc_key(preds[i]);
         vals[i] = __float_as_uint(load_target(target, tdtype, i));
     }
 }
 
 __global__ void pack_score_kernel(const float* __restrict__ preds, long long n, u64* __restrict__ keys, unsigned* __restrict__ vals) {
     for (long long i = blockIdx.x * (long long)kThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kThreads) {
-        keys[i] = score_key(preds[i]);
+        keys[i] = f32_desc_key(preds[i]);
         vals[i] = (unsigned)i;
     }
 }
@@ -181,7 +177,7 @@ __global__ void __launch_bounds__(kThreads) head_write_kernel(const u64* __restr
         if (is_head(keys, i, shift)) offsets[rank++] = i;
         if (perm) {
             const unsigned p = perm[i];
-            keys_out[i] = ((u64)(rank - 1) << 32) | score_key(preds[p]);
+            keys_out[i] = ((u64)(rank - 1) << 32) | f32_desc_key(preds[p]);
             tgt_out[i] = load_target(target, tdtype, p);
         }
     }
@@ -192,7 +188,7 @@ __global__ void pack_ideal_kernel(const u64* __restrict__ keys, const float* __r
                                   unsigned* __restrict__ out_vals) {
     for (long long i = blockIdx.x * (long long)kThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kThreads) {
         const float t = tgt[i];
-        out_keys[i] = (keys[i] & 0xffffffff00000000ull) | score_key(t);
+        out_keys[i] = (keys[i] & 0xffffffff00000000ull) | f32_desc_key(t);
         out_vals[i] = __float_as_uint(t);
     }
 }

@@ -27,8 +27,6 @@
 
 namespace mb200 {
 
-extern void count_launch();
-
 namespace {
 
 constexpr int kThreads = 256;
@@ -141,21 +139,21 @@ struct OH<Bool> {  // torch.bool: & and * are both the logical and
 template <>
 struct OH<float> {
     using A = double;
-    __device__ static A val(float x) { return x; }
+    __device__ static A val(float x) { return widen(x); }
     template <int OP>
     __device__ static A prod(float a, float b) { return __fmul_rn(a, b); }
 };
 template <>
 struct OH<__half> {  // the float product of two halves is exact; one rounding gives the half product
     using A = double;
-    __device__ static A val(__half x) { return __half2float(x); }
+    __device__ static A val(__half x) { return widen(x); }
     template <int OP>
     __device__ static A prod(__half a, __half b) { return __half2float(__float2half_rn(__fmul_rn(__half2float(a), __half2float(b)))); }
 };
 template <>
 struct OH<__nv_bfloat16> {
     using A = double;
-    __device__ static A val(__nv_bfloat16 x) { return __bfloat162float(x); }
+    __device__ static A val(__nv_bfloat16 x) { return widen(x); }
     template <int OP>
     __device__ static A prod(__nv_bfloat16 a, __nv_bfloat16 b) {
         return __bfloat162float(__float2bfloat16_rn(__fmul_rn(__bfloat162float(a), __bfloat162float(b))));
@@ -169,12 +167,6 @@ __device__ __forceinline__ void add3(T a, T b, typename OH<T>::A& ai, typename O
     at += OH<T>::val(b);
 }
 
-template <typename A>
-__device__ __forceinline__ A warp_sum(A v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-    return v;
-}
 __device__ __forceinline__ void emit(unsigned long long* p, unsigned long long v) {
     if (v != 0ull) atomicAdd(p, v);
 }

@@ -26,8 +26,6 @@
 
 namespace mb200 {
 
-extern void count_launch();
-
 namespace {
 
 constexpr int kThreads = 256;
@@ -36,53 +34,22 @@ constexpr int kTW = 32;                  // output columns of a tile: one per la
 constexpr int kRangeBlocks = 1024;       // CTAs of the data-range pass: its partials have a fixed size
 constexpr int kMaxSmem = 226 * 1024;     // dynamic shared memory of one CTA: sm_90's 227 KB less the static arrays
 
+// A: the compute type of T; kHalf: T is a 16-bit type; from_d: a double as `tensor.to(T)` converts it
 template <typename T>
-struct Cvt;
-template <>
-struct Cvt<float> {
-    using A = float;
-    static constexpr bool kHalf = false;
-    __device__ static float to_a(float v) { return v; }
-    __device__ static float from_f(float v) { return v; }
-    __device__ static float from_d(double v) { return (float)v; }
-    __device__ static float from_a(float v) { return v; }
-};
-template <>
-struct Cvt<double> {
-    using A = double;
-    static constexpr bool kHalf = false;
-    __device__ static double to_a(double v) { return v; }
-    __device__ static double from_f(float v) { return v; }
-    __device__ static double from_d(double v) { return v; }
-    __device__ static double from_a(double v) { return v; }
-};
-template <>
-struct Cvt<__half> {
-    using A = float;
-    static constexpr bool kHalf = true;
-    __device__ static float to_a(__half v) { return __half2float(v); }
-    __device__ static __half from_f(float v) { return __float2half_rn(v); }
-    __device__ static __half from_d(double v) { return __float2half_rn((float)v); }  // as torch: through float
-    __device__ static __half from_a(float v) { return __float2half_rn(v); }
-};
-template <>
-struct Cvt<__nv_bfloat16> {
-    using A = float;
-    static constexpr bool kHalf = true;
-    __device__ static float to_a(__nv_bfloat16 v) { return __bfloat162float(v); }
-    __device__ static __nv_bfloat16 from_f(float v) { return __float2bfloat16_rn(v); }
-    __device__ static __nv_bfloat16 from_d(double v) { return __float2bfloat16_rn((float)v); }
-    __device__ static __nv_bfloat16 from_a(float v) { return __float2bfloat16_rn(v); }
+struct Cvt {
+    using A = compute_t<T>;
+    static constexpr bool kHalf = sizeof(T) == 2;
+    __device__ static T from_d(double v) { return narrow<T>((A)v); }  // as torch: half / bfloat16 through float
 };
 
 // element i of a float tensor with tag `dtype`, converted to T as `tensor.to(T)` converts it
 template <typename T>
 __device__ __forceinline__ T load_as(const void* p, int dtype, long long i) {
     switch (dtype) {
-        case MB200_F32: return Cvt<T>::from_f(reinterpret_cast<const float*>(p)[i]);
+        case MB200_F32: return narrow<T>(reinterpret_cast<const float*>(p)[i]);
         case MB200_F64: return Cvt<T>::from_d(reinterpret_cast<const double*>(p)[i]);
-        case MB200_F16: return Cvt<T>::from_f(__half2float(reinterpret_cast<const __half*>(p)[i]));
-        default: return Cvt<T>::from_f(__bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p)[i]));
+        case MB200_F16: return narrow<T>(widen(reinterpret_cast<const __half*>(p)[i]));
+        default: return narrow<T>(widen(reinterpret_cast<const __nv_bfloat16*>(p)[i]));
     }
 }
 
@@ -118,11 +85,11 @@ __device__ __forceinline__ long long reflect(long long i, long long n) {
 template <typename T>
 __device__ __forceinline__ typename Cvt<T>::A load_px(const Vol& v, long long off, const Clamp& cl) {
     using A = typename Cvt<T>::A;
-    A a = Cvt<T>::to_a(load_as<T>(v.p, v.dtype, off));
+    A a = widen(load_as<T>(v.p, v.dtype, off));
     if (cl.on && !isnan(a)) {
         a = a < (A)cl.lo ? (A)cl.lo : a;  // torch.clamp: min(max(v, lo), hi) in the op math type, NaN kept
         a = a > (A)cl.hi ? (A)cl.hi : a;
-        if (Cvt<T>::kHalf) a = Cvt<T>::to_a(Cvt<T>::from_a(a));
+        if (Cvt<T>::kHalf) a = round_to<T>(a);
     }
     return a;
 }
@@ -143,11 +110,6 @@ template <typename T>
 struct Tile {
     static constexpr int kH = sizeof(typename Cvt<T>::A) == 8 ? 16 : 32;  // output rows of a tile
 };
-
-__device__ __forceinline__ double warp_sum(double v) {
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-    return v;
-}
 
 // ---- epilogues: what ssim_kernel makes of the moments of one output position ---------------------------------------
 // begin() runs once per CTA on its own copy; operator() takes the means, the clamped variances and the covariance of
@@ -267,7 +229,7 @@ __global__ void __launch_bounds__(kThreads, 2) ssim_kernel(Vol P, Vol Q, Geo g, 
     const int tid = threadIdx.x, lane = tid & 31, rg = tid >> 5;
     const long long baseP = bi * P.sn + ch * P.sc, baseQ = bi * Q.sn + ch * Q.sc;
 
-    for (int i = tid; i < kd + kh + kw; i += kThreads) wD[i] = Cvt<T>::to_a(weights[i]);
+    for (int i = tid; i < kd + kh + kw; i += kThreads) wD[i] = widen(weights[i]);
     __syncthreads();
     if (tid < 3) {
         // each axis's taps divided by their float64 sum: moments about a shift equal the reference's only for a filter
@@ -398,7 +360,7 @@ __global__ void __launch_bounds__(kThreads, 2) ssim_kernel(Vol P, Vol Q, Geo g, 
             const EpiOut<A> r = e(mx + sx, my + sy, vx, vy, acc[4][j] - mx * my, g, oh, ow);
             ssum += r.s0;
             csum += r.s1;
-            if (map) map[(((bi * g.c + ch) * g.od + od) * g.oh + oh) * g.ow + ow] = Cvt<T>::from_a(r.map);
+            if (map) map[(((bi * g.c + ch) * g.od + od) * g.oh + oh) * g.ow + ow] = narrow<T>(r.map);
         }
     }
     ssum = warp_sum(ssum);
@@ -511,8 +473,8 @@ __global__ void __launch_bounds__(kThreads) range_final_kernel(const typename Cv
     block_minmax<A>(v, red);
     if (threadIdx.x == 0) {
         // preds.max() - preds.min() in the preds dtype; Python's max(a, b) keeps a unless b > a
-        const A pr = Cvt<T>::to_a(Cvt<T>::from_a(v[1] - v[0]));
-        const A tr = Cvt<T>::to_a(Cvt<T>::from_a(v[3] - v[2]));
+        const A pr = round_to<T>(v[1] - v[0]);
+        const A tr = round_to<T>(v[3] - v[2]);
         const A r = tr > pr ? tr : pr;
         const A a = (A)k1 * r, b = (A)k2 * r;
         consts[MB200_SSIM_RANGE] = (double)r;
@@ -548,8 +510,8 @@ __global__ void __launch_bounds__(kThreads) pool_kernel(Vol P, Vol Q, Geo g, int
                     sp += load_px<T>(P, bi * P.sn + ci * P.sc + dz * P.sd + hy * P.sh + wx * P.sw, none);
                     sq += load_px<T>(Q, bi * Q.sn + ci * Q.sc + dz * Q.sd + hy * Q.sh + wx * Q.sw, none);
                 }
-        po[i] = Cvt<T>::from_a(sp / (A)(4 * fd));
-        qo[i] = Cvt<T>::from_a(sq / (A)(4 * fd));
+        po[i] = narrow<T>(sp / (A)(4 * fd));
+        qo[i] = narrow<T>(sq / (A)(4 * fd));
     }
 }
 
@@ -565,7 +527,7 @@ __global__ void __launch_bounds__(kThreads) decimate_kernel(Vol P, Vol Q, Geo g,
     const int kh = g.kh, kw = g.kw;
     A* wH = wt;
     A* wW = wt + kh;
-    for (int i = threadIdx.x; i < kh + kw; i += kThreads) wt[i] = Cvt<T>::to_a(weights[i]);
+    for (int i = threadIdx.x; i < kh + kw; i += kThreads) wt[i] = widen(weights[i]);
     __syncthreads();
     if (threadIdx.x < 2) {
         A* w = threadIdx.x == 0 ? wH : wW;
@@ -598,8 +560,8 @@ __global__ void __launch_bounds__(kThreads) decimate_kernel(Vol P, Vol Q, Geo g,
             sp += wH[a] * rp;
             sq += wH[a] * rq;
         }
-        po[i] = Cvt<T>::from_a(sp);
-        qo[i] = Cvt<T>::from_a(sq);
+        po[i] = narrow<T>(sp);
+        qo[i] = narrow<T>(sq);
     }
 }
 
