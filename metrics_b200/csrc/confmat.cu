@@ -53,8 +53,9 @@ constexpr int kRowThreads = 256;
 
 // (1) aligned path: warp per row, 16-byte streaming vector loads from global memory.  The label of the warp's NEXT
 // row is requested before the current row is reduced, so label latency never sits in front of the row loads.
-// With >= 4 resident CTAs/SM the reduction is meant to hide behind the HBM stream; tools/confmat_sweep.cu times this loop
+// With >= 4 resident CTAs/SM the reduction is meant to hide behind the HBM stream; tools/k1_budget.cu prices this loop
 // against a read-only streaming probe over the same 131 MB (DESIGN.md §K1 lists the alternatives that measured slower).
+// The grid is vec_grid's: one row per warp for rows of >= 1 KiB, else one resident wave.
 template <typename T, typename Sink, bool kI64>
 __global__ void __launch_bounds__(kRowThreads) rows_vec_kernel(RowArgs a, Sink sink) {
     // Let the next update's grid (launched with programmatic stream serialization, see launch_overlapped) start filling
@@ -238,6 +239,24 @@ static int resident_blocks(Kernel k, int threads, size_t smem) {
     return blocks;
 }
 
+// Grid of the vec path.  A one-wave grid-stride loop ends when its slowest SM ends.  One row per warp instead (a grid of
+// ceil(n / 8) CTAs) lets the hardware block scheduler hand the rows out as SMs free up, so all SMs drain together.  It pays
+// for rows of >= 1 KiB: [16384 | 65536, C] bf16 back-to-back updates on the H100 take 3.6 to 7.8 % less time at C = 512,
+// 768 and 1000 (cfg2: 43.4 instead of 44.9 us).  Shorter rows keep one wave: at 512 B (C = 256, 65536 rows) the two grids tie,
+// and at 256 B (C = 128, 262144 rows) one row per warp is 5.6 % slower (benchmarks/k1_budget.py, DESIGN.md §K1).  Sinks with
+// a per-CTA tail (Sink::kBlockTail: a shared-memory flush, per-warp totals into one word, a last-CTA ticket) pay it once
+// per CTA, so they keep one wave too.  rows_vec_kernel's int row index reaches (last row) + (warps in the grid), up to
+// 2 n + 6 on this grid, so launches of about 2^30 rows or more (over 1 TiB of logits at this row size) keep one wave as well.
+constexpr size_t kRowPerWarpMinBytes = 1024;
+
+template <typename Sink>
+static int vec_grid(long long n_rows, size_t row_bytes, int wave) {
+    constexpr int wpb = kRowThreads / kWarp;
+    if (Sink::kBlockTail || row_bytes < kRowPerWarpMinBytes || 2 * n_rows + 6 > INT_MAX)
+        return grid_for(n_rows, wpb, wave);
+    return grid_for(n_rows, wpb, INT_MAX);
+}
+
 template <typename T, typename Sink, bool kI64>
 static int launch_rows(const RowArgs& a, Sink sink, size_t smem, cudaStream_t st) {
     const size_t row_bytes = (size_t)a.C * sizeof(T);
@@ -246,7 +265,7 @@ static int launch_rows(const RowArgs& a, Sink sink, size_t smem, cudaStream_t st
     if (vec_ok) {
         if constexpr (sizeof(T) <= 4) {
             auto kern = rows_vec_kernel<T, Sink, kI64>;
-            const int grid = grid_for(a.n_outer, kRowThreads / 32, resident_blocks(kern, kRowThreads, smem));
+            const int grid = vec_grid<Sink>(a.n_outer, row_bytes, resident_blocks(kern, kRowThreads, smem));
             if constexpr (Sink::kOverlapSafe)
                 MB200_CUDA_OK(launch_overlapped(kern, grid, kRowThreads, smem, st, a, sink));
             else

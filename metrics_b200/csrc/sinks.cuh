@@ -16,6 +16,7 @@ struct ArgmaxOutSink {
     __device__ __forceinline__ void finish(Local&) {}
     static constexpr bool kNeedsTarget = false;
     static constexpr bool kOverlapSafe = false;
+    static constexpr bool kBlockTail = false;
 };
 
 // confmat[t, p] += 1 straight into the (L2-resident) state; optional shared-memory privatisation for tiny C.
@@ -28,6 +29,8 @@ struct ConfmatSink {
     // Two consecutive launches may overlap (programmatic dependent launch): all they share is the state, and they only
     // ever touch it with commutative 64-bit REDs.
     static constexpr bool kOverlapSafe = true;
+    // Each CTA zeroes and flushes its C*C shared-memory bins (see kBlockTail in confmat.cu).
+    static constexpr bool kBlockTail = kSmem;
     __device__ __forceinline__ void block_init() {
         if (kSmem) {
             extern __shared__ unsigned sh_bins[];
@@ -76,6 +79,8 @@ struct StatsSink {
     // issues commutative REDs, and its successor in the stream (the fold kernel) waits for it explicitly.  Its own
     // griddepcontrol.wait also orders its REDs after the previous update's fold, which re-zeroes this workspace.
     static constexpr bool kOverlapSafe = kDeferFold;
+    // Every warp REDs its totals into ONE word, and (unless deferred) every CTA pays a fence + ticket.
+    static constexpr bool kBlockTail = true;
     __device__ __forceinline__ void block_init() {
         if (kSmem) {
             extern __shared__ unsigned sh_bins[];
@@ -212,6 +217,7 @@ struct SamplewiseSink {
     struct Local {};
     static constexpr bool kNeedsTarget = true;
     static constexpr bool kOverlapSafe = false;
+    static constexpr bool kBlockTail = false;
     __device__ __forceinline__ void block_init() {}
     __device__ __forceinline__ void init(Local&) {}
     __device__ __forceinline__ void row(Local&, long long idx, long long t, int p) {
